@@ -1106,7 +1106,6 @@ static int pass_front(pa_agg* a) {
   cudaStream_t s = a->s_comp;
   Counters* ctr = a->d_ctr.as<Counters>();
   StackSlot* tab = a->d_table.as<StackSlot>();
-  const int G = a->G;
   CK(cudaEventRecord(a->tm[T_TOTAL].a, s));
   CK(cudaMemsetAsync(ctr, 0, sizeof(Counters), s));
   CK(cudaMemsetAsync(tab, 0, (P.cap + 2) * sizeof(StackSlot), s));
@@ -1133,7 +1132,7 @@ static int pass_front(pa_agg* a) {
     }
     h.first_kind = P.v1 ? a->v1_first_kind : nullptr;
     uint64_t rows = r1 - r0;
-    int hb = (int)std::min<uint64_t>((rows + kThreads - 1) / kThreads, (uint64_t)G * 2);
+    int hb = (int)std::min<uint64_t>((rows + kThreads - 1) / kThreads, (uint64_t)a->sms * kHdrBlocksPerSm);
     k_header<<<std::max(hb, 1), kThreads, 0, s>>>(h);
     a->tm[T_HEADER].launches++;
   };
