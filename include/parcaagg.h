@@ -77,6 +77,7 @@ enum {
 
 #define PA_IPC_PLAIN 0u
 #define PA_IPC_LZ4_FRAME 1u
+#define PA_IPC_LZ4_FRAME_GPU 2u
 
 #define PA_CFG_SINGLE_RING 0x1u /* one ring buffer instead of two: ingest is refused (PA_ENOSPC) while a flush holds the ring.
                                     Halves the pinned host memory; for replay / batch use, not for a live agent */
@@ -155,7 +156,13 @@ typedef struct pa_agg_config {
                                   then take and hand out uint32 arrays through the same pointers. */
   uint32_t ipc_compression;    /* PA_IPC_PLAIN (0): uncompressed bodies == the offline-mode bytes (:1779-1790), the bit-exact mode.
                                   PA_IPC_LZ4_FRAME (1): bodies wrapped like ipc.WithLZ4() (:1851, the gRPC path) — decodes to the
-                                  same record but is NOT byte-identical to the Go writer (different LZ4 encoder) */
+                                  same record but is NOT byte-identical to the Go writer (different LZ4 encoder). Host work: the
+                                  uncompressed stream is copied out, then re-encoded with the system liblz4.so.1.
+                                  PA_IPC_LZ4_FRAME_GPU (2): the same framing (ipc.WithLZ4()), with the bodies encoded on the GPU in
+                                  independent 64 KiB LZ4 blocks; only the compressed bodies cross PCIe and no liblz4 is needed. It
+                                  decodes to the same record and is NOT byte-identical to the Go writer (nor to mode 1). The mode for
+                                  the gRPC path. Both modes apply to every result: v2 and v1 sample records and pa_agg_stacktraces.
+                                  Merge groups never compress: pa_merge_create_* refuse a PA_IPC_LZ4_FRAME_GPU member (PA_EINVAL). */
 } pa_agg_config;
 
 /* Result of one flush; memory is library-owned (pinned host) until pa_agg_release. */
@@ -220,7 +227,8 @@ int pa_agg_stage(pa_agg* a);
 int pa_agg_process(pa_agg* a);
 int pa_agg_collect(pa_agg* a, pa_agg_result* out);
 /* device time (ms, CUDA events on the compute stream) of named kernel groups during the last
- * process(): names are "hash", "header", "rank", "locations", "labels", "dicts", "total". Two more names report counters of the
+ * process(): names are "hash", "header", "rank", "locations", "labels", "dicts", "total". "lz4" reports the compression kernels of
+ * the last collect / pa_agg_stacktraces in PA_IPC_LZ4_FRAME_GPU mode. Two more names report counters of the
  * v1 stack store since creation in *launches (ms = 0): "store_compactions", "store_evictions". */
 int pa_agg_last_kernel_ms(const pa_agg* a, const char* name, double* ms, uint32_t* launches);
 /* copies the per-row 128-bit stack ids (big-endian hi‖lo, 16 B per row) of the staged batch. */

@@ -21,7 +21,7 @@ PA_XXH_SEED_LO = 0x9E3779B97F4A7C15
 
 PA_LABEL_DISABLE_CPU, PA_LABEL_DISABLE_THREAD_ID, PA_LABEL_DISABLE_THREAD_COMM = 1, 2, 4
 PA_SCHEMA_V2, PA_SCHEMA_V1 = 0, 1
-PA_IPC_PLAIN, PA_IPC_LZ4_FRAME = 0, 1
+PA_IPC_PLAIN, PA_IPC_LZ4_FRAME, PA_IPC_LZ4_FRAME_GPU = 0, 1, 2
 PA_NO_STRING = 0xFFFFFFFF
 
 # struct pa_sample_hdr (64 B)

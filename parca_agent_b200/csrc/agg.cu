@@ -92,8 +92,8 @@ struct Timer {
   uint32_t launches = 0;
   double ms = 0;
 };
-static const char* kTimerNames[] = {"header", "hash", "rank", "locations", "labels", "dicts", "total"};
-enum { T_HEADER, T_HASH, T_RANK, T_LOC, T_LABELS, T_DICTS, T_TOTAL, T_COUNT };
+static const char* kTimerNames[] = {"header", "hash", "rank", "locations", "labels", "dicts", "total", "lz4"};
+enum { T_HEADER, T_HASH, T_RANK, T_LOC, T_LABELS, T_DICTS, T_TOTAL, T_LZ4 /* collect / stacktraces, not process */, T_COUNT };
 
 }  // namespace pa
 
@@ -244,6 +244,8 @@ struct pa_agg {
   size_t h_desc_cap = 0;
   std::vector<std::vector<uint8_t>> hostbufs;  // host-built Arrow buffers of the current result
   std::vector<uint8_t> comp_out;               // PA_IPC_LZ4_FRAME: the re-encoded stream the result points at
+  DBuf d_lz4, d_lz4_body;                      // PA_IPC_LZ4_FRAME_GPU: block tables, host-source staging and block slots; compressed bodies
+  cudaEvent_t ev_lz4p0 = nullptr, ev_lz4p1 = nullptr;  // around k_lz4_pack (T_LZ4 covers compress + layout)
   Timer tm[T_COUNT];
   uint32_t launches = 0;
   double h2d_ms = 0;
@@ -371,7 +373,7 @@ uint32_t pa_agg_abi_version(void) { return PA_ABI_VERSION; }
 const char* pa_agg_last_error(const pa_agg* a) { return a ? a->err.c_str() : "null handle"; }
 
 int pa_agg_create(const pa_agg_config* cfg, pa_agg** out) {
-  if (!cfg || !out || cfg->abi_version != PA_ABI_VERSION || cfg->samples_per_second == 0 || cfg->max_samples == 0 || cfg->hash_mode > 1 || cfg->schema > 1 || cfg->ipc_compression > 1 ||
+  if (!cfg || !out || cfg->abi_version != PA_ABI_VERSION || cfg->samples_per_second == 0 || cfg->max_samples == 0 || cfg->hash_mode > 1 || cfg->schema > 1 || cfg->ipc_compression > PA_IPC_LZ4_FRAME_GPU ||
       (cfg->frame_id_bytes != 0 && cfg->frame_id_bytes != 4 && cfg->frame_id_bytes != 8)) return PA_EINVAL;
   if (cfg->max_samples > 0x7FFFFFFFull) return PA_ERANGE;  // run ends / ListView offsets are int32
   int ndev = 0;
@@ -444,6 +446,7 @@ int pa_agg_create(const pa_agg_config* cfg, pa_agg** out) {
   cudaEventCreate(&a->ev_d2h0);
   cudaEventCreate(&a->ev_d2h1);
   for (int t = 0; t < T_COUNT; t++) { cudaEventCreate(&a->tm[t].a); cudaEventCreate(&a->tm[t].b); }
+  if (a->cfg.ipc_compression == PA_IPC_LZ4_FRAME_GPU) { cudaEventCreate(&a->ev_lz4p0); cudaEventCreate(&a->ev_lz4p1); }
   const uint64_t N = a->cfg.max_samples, NF = a->cfg.max_frames;
   if (a->idb == 4 && a->hash_variant != 5) a->hash_variant = 2;  // (the tma variants fall through to wide32 in launch_hash)  // the narrow ring is read by the `wide` kernel (widening loads); the other variants take uint64 ids
   for (int r = 0; r < (a->single_ring ? 1 : 2); r++) {
@@ -512,13 +515,15 @@ void pa_agg_destroy(pa_agg* a) {
                  &a->d_arena, &a->d_partial, &a->d_partial2, &a->d_ree_partial, &a->d_lsmat, &a->d_kindtab, &a->d_cols, &a->d_jobs,
                  &a->m_addr.buf, &a->m_line.buf, &a->m_type.buf, &a->m_map.buf, &a->m_bid.buf, &a->m_func.buf, &a->m_fnfile.buf, &a->m_sid2cid.buf,
                  &a->m1_map.buf, &a->m1_bid.buf, &a->m1_fn.buf, &a->m1_file.buf, &a->m1_line.buf, &a->m1_col.buf, &a->m1_complete.buf,
-                 &a->d_store, &a->d_store_arena, &a->d_store_ctl, &a->d_v1_ids, &a->d_st1, &a->d_store_stamp, &a->d_v1_last, &a->d_select};
+                 &a->d_store, &a->d_store_arena, &a->d_store_ctl, &a->d_v1_ids, &a->d_st1, &a->d_store_stamp, &a->d_v1_last, &a->d_select, &a->d_lz4, &a->d_lz4_body};
   for (DBuf* b : all) b->release();
   for (auto e : a->chunk_ev) cudaEventDestroy(e);
   if (a->ev_h2d0) cudaEventDestroy(a->ev_h2d0);
   if (a->ev_h2d1) cudaEventDestroy(a->ev_h2d1);
   if (a->ev_d2h0) cudaEventDestroy(a->ev_d2h0);
   if (a->ev_d2h1) cudaEventDestroy(a->ev_d2h1);
+  if (a->ev_lz4p0) cudaEventDestroy(a->ev_lz4p0);
+  if (a->ev_lz4p1) cudaEventDestroy(a->ev_lz4p1);
   for (int t = 0; t < T_COUNT; t++) { if (a->tm[t].a) cudaEventDestroy(a->tm[t].a); if (a->tm[t].b) cudaEventDestroy(a->tm[t].b); }
   if (a->ev_fork) cudaEventDestroy(a->ev_fork);
   if (a->ev_join) cudaEventDestroy(a->ev_join);
@@ -644,7 +649,8 @@ static int stage_async(pa_agg* a) {
   a->early = pa_agg::Early{};
   // headers first when the frame ids take several chunks: everything that depends only on the headers (k_header, the label chain,
   // the early copy-out) then overlaps the upload of the ids
-  a->early.hdr_first = a->early_enabled && nchunks > 1 && a->cfg.hash_mode == PA_HASH_XXH64X2 && a->cfg.schema != PA_SCHEMA_V1 && !a->serial;
+  // (the compressed stream's layout is only known once its bodies are encoded: PA_IPC_LZ4_FRAME_GPU has no early copy-out)
+  a->early.hdr_first = a->early_enabled && a->cfg.ipc_compression != PA_IPC_LZ4_FRAME_GPU && nchunks > 1 && a->cfg.hash_mode == PA_HASH_XXH64X2 && a->cfg.schema != PA_SCHEMA_V1 && !a->serial;
   if (a->early.hdr_first) {
     CK(cudaMemcpyAsync(a->d_hdr.p, r.hdr, a->N * 64, cudaMemcpyHostToDevice, a->s_copy));
     CK(cudaEventRecord(a->ev_hdr_all, a->s_copy));
@@ -1861,6 +1867,123 @@ static int early_copy_issue(pa_agg* a) {
   return PA_OK;
 }
 
+// PA_IPC_LZ4_FRAME_GPU: writes the stream `plan` describes to a->out with every record and dictionary batch body compressed
+// on the device (the framing of ipc_compress_lz4; only the compressed bodies cross PCIe). The host assembles the metadata with
+// the same rewrite as the host mode, from the per-buffer frame sizes. *d2h_ms: the copy-out of the bodies.
+static int lz4_gpu_stream(pa_agg* a, const StreamPlan& plan, cudaStream_t s, uint64_t* out_len, float* d2h_ms) {
+  const size_t M = plan.messages.size();
+  std::vector<BatchMeta> meta(M);
+  std::vector<uint32_t> buf0(M, 0);  // first entry of each message's buffers in `bufs`
+  std::vector<Lz4Blk> blks;
+  std::vector<Lz4Buf> bufs;
+  std::vector<uint8_t> staged;                              // HOST sources, uploaded with one copy
+  std::vector<std::pair<size_t, uint64_t>> staged_blk;      // (block, its offset in `staged`)
+  std::string why;
+  for (size_t m = 1; m < M; m++) {  // message 0 is the schema (copied verbatim)
+    const StreamPlan::Message& g = plan.messages[m];
+    const std::vector<uint8_t>& blob = plan.message_meta(m);
+    if (!read_batch_meta(blob.data() + 8, (uint32_t)blob.size() - 8, &meta[m], &why)) return a->fail(PA_EIO, why.c_str());
+    if (meta[m].buffers.size() != 2 * (g.p1 - g.p0)) return a->fail(PA_EIO, "stream plan and batch metadata disagree");
+    buf0[m] = (uint32_t)bufs.size();
+    for (size_t i = g.p0; i < g.p1; i++) {
+      const BufRef& r = plan.placements[i].src;
+      if (r.len && r.kind != BufRef::DEVICE && r.kind != BufRef::HOST && r.kind != BufRef::ZEROS) return a->fail(PA_EINVAL, "buffer without a source");
+      bufs.push_back(Lz4Buf{r.len, (uint32_t)blks.size(), (uint32_t)((r.len + kLz4Block - 1) / kLz4Block)});
+      for (uint64_t o = 0; o < r.len; o += kLz4Block) {
+        if (r.kind == BufRef::HOST) staged_blk.emplace_back(blks.size(), staged.size() + o);
+        blks.push_back(Lz4Blk{r.kind == BufRef::DEVICE ? (const uint8_t*)r.ptr + o : nullptr, (uint32_t)std::min<uint64_t>(kLz4Block, r.len - o), (uint32_t)bufs.size() - 1});
+      }
+      if (r.kind == BufRef::HOST && r.len) staged.insert(staged.end(), (const uint8_t*)r.ptr, (const uint8_t*)r.ptr + r.len);
+    }
+  }
+  const size_t nb = blks.size(), nbuf = bufs.size();
+  auto al = [](size_t v) { return (v + 255) & ~(size_t)255; };
+  const size_t o_bufs = al(nb * sizeof(Lz4Blk)), o_size = o_bufs + al(nbuf * sizeof(Lz4Buf)), o_off = o_size + al(nb * 4), o_frame = o_off + al(nb * 8),
+               o_dst = o_frame + al(nbuf * 8), o_staged = o_dst + al(nbuf * 8), o_slots = o_staged + al(staged.size()), bytes = o_slots + nb * kLz4Block;
+  CK(a->d_lz4.ensure(std::max<size_t>(bytes, 256)));
+  uint8_t* d = a->d_lz4.as<uint8_t>();
+  for (auto& hb : staged_blk) blks[hb.first].src = d + o_staged + hb.second;
+  Lz4Blk* d_blks = (Lz4Blk*)d;
+  Lz4Buf* d_bufs = (Lz4Buf*)(d + o_bufs);
+  uint32_t* d_size = (uint32_t*)(d + o_size);
+  uint64_t *d_off = (uint64_t*)(d + o_off), *d_frame = (uint64_t*)(d + o_frame), *d_dst = (uint64_t*)(d + o_dst);
+  if (nb) CK(cudaMemcpyAsync(d_blks, blks.data(), nb * sizeof(Lz4Blk), cudaMemcpyHostToDevice, s));
+  if (nbuf) CK(cudaMemcpyAsync(d_bufs, bufs.data(), nbuf * sizeof(Lz4Buf), cudaMemcpyHostToDevice, s));
+  if (!staged.empty()) CK(cudaMemcpyAsync(d + o_staged, staged.data(), staged.size(), cudaMemcpyHostToDevice, s));
+  Timer& t = a->tm[T_LZ4];
+  t.launches = 0;
+  CK(cudaEventRecord(t.a, s));
+  if (nb) { k_lz4_compress<<<(unsigned)((nb + kLz4Warps - 1) / kLz4Warps), kLz4Warps * 32, 0, s>>>(d_blks, (uint32_t)nb, d + o_slots, d_size); t.launches++; }
+  if (nbuf) { k_lz4_layout<<<(unsigned)((nbuf + kWarps - 1) / kWarps), kThreads, 0, s>>>(d_bufs, (uint32_t)nbuf, d_size, d_off, d_frame); t.launches++; }
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(t.b, s));
+  std::vector<uint64_t> frame(nbuf);
+  if (nbuf) CK(cudaMemcpyAsync(frame.data(), d_frame, nbuf * 8, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+
+  // ---- layout: a buffer is its int64 length and its frame, or -1 and its raw bytes when the frame is not smaller
+  std::vector<std::vector<uint8_t>> metas(M);
+  std::vector<uint64_t> body_dev(M, 0), body_len(M, 0), at(M, 0), dst(nbuf, 0);
+  uint64_t dev_total = 0, total = 0;
+  for (size_t m = 0; m < M; m++) {
+    if (m == 0) {
+      metas[m] = plan.message_meta(0);
+    } else {
+      const size_t n = plan.messages[m].p1 - plan.messages[m].p0;
+      std::vector<int64_t> sizes(n), offs;
+      for (size_t i = 0; i < n; i++) {
+        const Lz4Buf& B = bufs[buf0[m] + i];
+        sizes[i] = B.len ? 8 + (int64_t)std::min<uint64_t>(frame[buf0[m] + i], B.len) : 0;
+      }
+      int64_t bl = 0;
+      metas[m] = lz4_batch_message(meta[m], sizes, &offs, &bl);
+      for (size_t i = 0; i < n; i++) {
+        const Lz4Buf& B = bufs[buf0[m] + i];
+        dst[buf0[m] + i] = (dev_total + (uint64_t)offs[i]) | (B.len && frame[buf0[m] + i] >= B.len ? 1ull << 63 : 0);
+      }
+      body_dev[m] = dev_total;
+      body_len[m] = (uint64_t)bl;
+      dev_total += (uint64_t)bl;
+    }
+    at[m] = total;
+    total += metas[m].size() + body_len[m];
+  }
+  total += 8;
+  CK(a->d_lz4_body.ensure(std::max<uint64_t>(dev_total, 256)));
+  if (nbuf) CK(cudaMemcpyAsync(d_dst, dst.data(), nbuf * 8, cudaMemcpyHostToDevice, s));
+  CK(cudaEventRecord(a->ev_lz4p0, s));
+  if (nb) {
+    k_lz4_pack<<<(unsigned)((nb + kWarps - 1) / kWarps), kThreads, 0, s>>>(d_blks, (uint32_t)nb, d_bufs, d + o_slots, d_size, d_off, d_frame, d_dst, a->d_lz4_body.as<uint8_t>());
+    t.launches++;
+  }
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(a->ev_lz4p1, s));
+  if (total > a->out_cap) {
+    CK(cudaStreamSynchronize(a->s_d2h));
+    if (a->out) cudaFreeHost(a->out);
+    a->out = nullptr;
+    a->out_cap = 0;
+    uint64_t want = total + total / 4 + 4096;
+    if (cudaHostAlloc((void**)&a->out, want, cudaHostAllocDefault) != cudaSuccess) return a->fail(PA_ENOMEM, "pinned output allocation failed");
+    a->out_cap = want;
+  }
+  CK(cudaEventRecord(a->ev_d2h0, s));
+  for (size_t m = 0; m < M; m++)
+    if (body_len[m]) CK(cudaMemcpyAsync(a->out + at[m] + metas[m].size(), a->d_lz4_body.as<uint8_t>() + body_dev[m], body_len[m], cudaMemcpyDeviceToHost, s));
+  CK(cudaEventRecord(a->ev_d2h1, s));
+  for (size_t m = 0; m < M; m++) memcpy(a->out + at[m], metas[m].data(), metas[m].size());
+  const uint32_t eos[2] = {0xFFFFFFFFu, 0u};
+  memcpy(a->out + total - 8, eos, 8);
+  CK(cudaStreamSynchronize(s));
+  float ms = 0, pack = 0;
+  cudaEventElapsedTime(&ms, t.a, t.b);
+  cudaEventElapsedTime(&pack, a->ev_lz4p0, a->ev_lz4p1);
+  t.ms = (double)ms + pack;
+  cudaEventElapsedTime(d2h_ms, a->ev_d2h0, a->ev_d2h1);
+  *out_len = total;
+  return PA_OK;
+}
+
 static int collect(pa_agg* a, pa_agg_result* res) {
   memset(res, 0, sizeof *res);
   if (!a->processed) return a->fail(PA_EINVAL, "collect before process");
@@ -1905,6 +2028,17 @@ static int collect(pa_agg* a, pa_agg_result* res) {
   StreamPlan plan;
   plan.build(cols, {{"parca_write_schema_version", v1 ? "v1" : "v2"}}, (int64_t)N);
   const double t_plan = now_ms();
+  if (a->cfg.ipc_compression == PA_IPC_LZ4_FRAME_GPU) {
+    uint64_t len = 0;
+    float d2h = 0, h2d = 0;
+    if (int rc = lz4_gpu_stream(a, plan, a->s_comp, &len, &d2h)) return rc;
+    cudaEventElapsedTime(&h2d, a->ev_h2d0, a->ev_h2d1);
+    res->ipc = a->out; res->ipc_len = len; res->n_rows = N; res->n_unique_stacks = c.n_unique; res->n_locations = c.n_locations;
+    res->n_functions = c.n_functions; res->n_location_indices = (uint32_t)c.n_indices64; res->gpu_launches = a->launches;
+    res->h2d_ms = h2d; res->gpu_ms = a->tm[T_TOTAL].ms; res->d2h_ms = d2h; res->host_ms = std::max(0.0, now_ms() - t0 - d2h - a->tm[T_LZ4].ms);
+    release_staged(a);
+    return PA_OK;
+  }
   if (plan.total > a->out_cap) {
     if (a->early.issued) { CK(cudaStreamSynchronize(a->s_d2h)); a->early.issued = false; }  // the early copies went into the buffer that is too small
     if (a->out) cudaFreeHost(a->out);
@@ -2163,6 +2297,16 @@ static int stacktraces(pa_agg* a, const uint8_t* ids, uint64_t n, pa_agg_result*
 
   StreamPlan plan;
   plan.build(cols, {{"parca_write_schema_version", "v1"}}, (int64_t)n);
+  if (a->cfg.ipc_compression == PA_IPC_LZ4_FRAME_GPU) {
+    uint64_t len = 0;
+    float d2h = 0, gpu = 0;
+    if (int rc = lz4_gpu_stream(a, plan, s, &len, &d2h)) return rc;
+    cudaEventElapsedTime(&gpu, a->tm[T_TOTAL].a, a->tm[T_TOTAL].b);
+    res->ipc = a->out; res->ipc_len = len; res->n_rows = n; res->n_unique_stacks = n; res->n_locations = L; res->n_functions = c.n_dict[4];
+    res->n_location_indices = NL; res->gpu_launches = tm.launches; res->gpu_ms = gpu; res->d2h_ms = d2h;
+    res->host_ms = std::max(0.0, (now_ms() - t0) - gpu - d2h - a->tm[T_LZ4].ms);
+    return PA_OK;
+  }
   if (plan.total > a->out_cap) {
     CK(cudaStreamSynchronize(a->s_d2h));
     if (a->out) cudaFreeHost(a->out);

@@ -10,7 +10,8 @@
 // Input: any uncompressed stream this library wrote (schema, dictionary batches, one record batch, end marker).
 // The flatbuffer metadata is re-read with a few lines of table walking and rebuilt with pa::FlatBuilder, in the same
 // construction order as ipc_out.hpp (plus the `compression` field), so a stream compressed here and the oracle's stream
-// compressed by the same function stay comparable.
+// compressed by the same function stay comparable. The metadata rewrite (read_batch_meta + lz4_batch_message) is shared with
+// PA_IPC_LZ4_FRAME_GPU, which compresses the bodies on the device (k_lz4_* in kernels.cuh, lz4_gpu_stream in agg.cu).
 #pragma once
 #include <dlfcn.h>
 
@@ -89,6 +90,80 @@ struct Buf {  // one metadata flatbuffer; positions are byte offsets (0 = "absen
 };
 }  // namespace fbread
 
+// Metadata of one record batch (type 3) or dictionary batch (type 2) message.
+struct BatchMeta {
+  uint8_t type = 0;
+  int64_t length = 0, dict_id = 0;
+  std::vector<int64_t> nodes, buffers, variadic;  // buffers: (offset, length) pairs of the uncompressed body
+};
+
+// Reads the Message flatbuffer `meta` of a record or dictionary batch. False (and *err) on malformed or compressed metadata.
+inline bool read_batch_meta(const uint8_t* meta, uint32_t meta_len, BatchMeta* p, std::string* err) {
+  fbread::Buf fb{meta, meta_len};
+  int64_t m = fb.root();
+  p->type = fb.byte(fb.field(m, 1));
+  int64_t rb = fb.indirect(fb.field(m, 2));
+  if (!m || fb.bad || !rb || (p->type != 2 && p->type != 3)) { *err = "message without header"; return false; }
+  if (p->type == 2) {  // DictionaryBatch{id, data}
+    p->dict_id = fb.scalar64(fb.field(rb, 0));
+    rb = fb.indirect(fb.field(rb, 1));
+    if (!rb) { *err = "dictionary batch without data"; return false; }
+  }
+  p->length = fb.scalar64(fb.field(rb, 0));
+  bool vec_ok = fb.longs(fb.field(rb, 1), 2, &p->nodes) && fb.longs(fb.field(rb, 2), 2, &p->buffers) && fb.longs(fb.field(rb, 4), 1, &p->variadic);
+  if (!vec_ok || fb.bad) { *err = "malformed record batch metadata"; return false; }
+  if (fb.field(rb, 3)) { *err = "stream is already compressed"; return false; }
+  return true;
+}
+
+// The encapsulated metadata (continuation marker, length, flatbuffer, zero padding to 8 bytes) of `p` with
+// BodyCompression{LZ4_FRAME, BUFFER}, whose buffers hold sizes[b] bytes each (0 = empty), back to back at 8-byte aligned
+// offsets. *offs receives each buffer's offset in the new body and *body_len the body's length.
+inline std::vector<uint8_t> lz4_batch_message(const BatchMeta& p, const std::vector<int64_t>& sizes, std::vector<int64_t>* offs, int64_t* body_len) {
+  std::vector<int64_t> nb(p.buffers.size());
+  offs->assign(sizes.size(), 0);
+  int64_t at = 0;
+  for (size_t b = 0; b < sizes.size(); b++) {
+    (*offs)[b] = nb[2 * b] = at;
+    nb[2 * b + 1] = sizes[b];
+    at = (at + sizes[b] + 7) & ~(int64_t)7;
+  }
+  *body_len = at;
+  FlatBuilder fb;
+  uint32_t var = p.variadic.empty() ? 0 : fb.longs(p.variadic, 1);
+  fb.begin(2);                      // BodyCompression{codec = LZ4_FRAME (0), method = BUFFER (0)}: all defaults
+  uint32_t comp = fb.end();
+  uint32_t bufs = fb.longs(nb, 2);
+  uint32_t nodes = fb.longs(p.nodes, 2);
+  fb.begin(5);
+  fb.field<int64_t>(0, p.length, 0);
+  fb.ref(1, nodes);
+  fb.ref(2, bufs);
+  fb.ref(3, comp);
+  fb.ref(4, var);
+  uint32_t rb = fb.end();
+  uint32_t header = rb;
+  if (p.type == 2) {
+    fb.begin(3);
+    fb.field<int64_t>(0, p.dict_id, 0);
+    fb.ref(1, rb);
+    header = fb.end();
+  }
+  fb.begin(5);
+  fb.field<int16_t>(0, 4, 0);  // MetadataVersion V5
+  fb.field<uint8_t>(1, p.type, 0);
+  fb.ref(2, header);
+  fb.field<int64_t>(3, at, 0);
+  uint32_t m = fb.end();
+  fb.finish(m);
+  uint32_t n = fb.size(), padded = ((n + 8 + 7) & ~7u) - 8;
+  std::vector<uint8_t> out(8 + (size_t)padded, 0);
+  uint32_t pre[2] = {0xFFFFFFFFu, padded};
+  memcpy(out.data(), pre, 8);
+  memcpy(out.data() + 8, fb.data(), n);
+  return out;
+}
+
 // Re-encodes `in` with LZ4_FRAME body compression into `out`. Returns false and sets *err on malformed input / missing liblz4.
 inline bool ipc_compress_lz4(const uint8_t* in, uint64_t len, std::vector<uint8_t>& out, std::string* err, unsigned threads = 0) {
   static Lz4Api api;
@@ -118,28 +193,15 @@ inline bool ipc_compress_lz4(const uint8_t* in, uint64_t len, std::vector<uint8_
 
   // one task per non-empty buffer
   struct Task { const uint8_t* src; int64_t n; std::vector<uint8_t> dst; };
-  struct Plan { int64_t length = 0, dict_id = 0; bool is_dict = false; std::vector<int64_t> nodes, buffers, variadic; std::vector<int> task_of_buffer; };
+  struct Plan { BatchMeta meta; std::vector<int> task_of_buffer; };
   std::vector<Task> tasks;
   std::vector<Plan> plans(msgs.size());
   for (size_t i = 0; i < msgs.size(); i++) {
     if (msgs[i].type != 2 && msgs[i].type != 3) continue;
-    fbread::Buf fb{msgs[i].meta, msgs[i].meta_len};
-    int64_t m = fb.root();
-    int64_t rb = fb.indirect(fb.field(m, 2));
-    if (!rb) { *err = "message without header"; return false; }
     Plan& p = plans[i];
-    if (msgs[i].type == 2) {  // DictionaryBatch{id, data}
-      p.is_dict = true;
-      p.dict_id = fb.scalar64(fb.field(rb, 0));
-      rb = fb.indirect(fb.field(rb, 1));
-      if (!rb) { *err = "dictionary batch without data"; return false; }
-    }
-    p.length = fb.scalar64(fb.field(rb, 0));
-    bool vec_ok = fb.longs(fb.field(rb, 1), 2, &p.nodes) && fb.longs(fb.field(rb, 2), 2, &p.buffers) && fb.longs(fb.field(rb, 4), 1, &p.variadic);
-    if (!vec_ok || fb.bad) { *err = "malformed record batch metadata"; return false; }
-    if (fb.field(rb, 3)) { *err = "stream is already compressed"; return false; }
-    for (size_t b = 0; b + 1 < p.buffers.size(); b += 2) {
-      int64_t off = p.buffers[b], n = p.buffers[b + 1];
+    if (!read_batch_meta(msgs[i].meta, msgs[i].meta_len, &p.meta, err)) return false;
+    for (size_t b = 0; b + 1 < p.meta.buffers.size(); b += 2) {
+      int64_t off = p.meta.buffers[b], n = p.meta.buffers[b + 1];
       if (off < 0 || n < 0 || off > msgs[i].body_len || n > msgs[i].body_len - off) { *err = "buffer outside its body"; return false; }
       if (n == 0) { p.task_of_buffer.push_back(-1); continue; }
       p.task_of_buffer.push_back((int)tasks.size());
@@ -179,49 +241,15 @@ inline bool ipc_compress_lz4(const uint8_t* in, uint64_t len, std::vector<uint8_
       continue;
     }
     Plan& p = plans[i];
-    std::vector<int64_t> nb(p.buffers.size());
-    std::vector<uint8_t> body;
-    for (size_t b = 0; b < p.task_of_buffer.size(); b++) {
-      nb[2 * b] = (int64_t)body.size();
-      int t = p.task_of_buffer[b];
-      nb[2 * b + 1] = t < 0 ? 0 : (int64_t)tasks[t].dst.size();
-      if (t >= 0) body.insert(body.end(), tasks[t].dst.begin(), tasks[t].dst.end());
-      body.resize((body.size() + 7) & ~(size_t)7, 0);
-    }
-    FlatBuilder fb;
-    uint32_t var = p.variadic.empty() ? 0 : fb.longs(p.variadic, 1);
-    fb.begin(2);                      // BodyCompression{codec = LZ4_FRAME (0), method = BUFFER (0)}: all defaults
-    uint32_t comp = fb.end();
-    uint32_t bufs = fb.longs(nb, 2);
-    uint32_t nodes = fb.longs(p.nodes, 2);
-    fb.begin(5);
-    fb.field<int64_t>(0, p.length, 0);
-    fb.ref(1, nodes);
-    fb.ref(2, bufs);
-    fb.ref(3, comp);
-    fb.ref(4, var);
-    uint32_t rb = fb.end();
-    uint32_t header = rb;
-    if (p.is_dict) {
-      fb.begin(3);
-      fb.field<int64_t>(0, p.dict_id, 0);
-      fb.ref(1, rb);
-      header = fb.end();
-    }
-    fb.begin(5);
-    fb.field<int16_t>(0, 4, 0);  // MetadataVersion V5
-    fb.field<uint8_t>(1, msgs[i].type, 0);
-    fb.ref(2, header);
-    fb.field<int64_t>(3, (int64_t)body.size(), 0);
-    uint32_t m = fb.end();
-    fb.finish(m);
-    uint32_t n = fb.size(), padded = ((n + 8 + 7) & ~7u) - 8;
-    uint32_t pre[2] = {0xFFFFFFFFu, padded};
-    append(pre, 8);
-    append(fb.data(), n);
-    static const uint8_t z[8] = {0};
-    append(z, padded - n);
-    append(body.data(), body.size());
+    std::vector<int64_t> sizes(p.task_of_buffer.size()), offs;
+    for (size_t b = 0; b < sizes.size(); b++) sizes[b] = p.task_of_buffer[b] < 0 ? 0 : (int64_t)tasks[p.task_of_buffer[b]].dst.size();
+    int64_t body_len = 0;
+    std::vector<uint8_t> meta = lz4_batch_message(p.meta, sizes, &offs, &body_len);
+    append(meta.data(), meta.size());
+    size_t body = out.size();
+    out.resize(body + (size_t)body_len, 0);
+    for (size_t b = 0; b < sizes.size(); b++)
+      if (sizes[b]) memcpy(out.data() + body + offs[b], tasks[p.task_of_buffer[b]].dst.data(), (size_t)sizes[b]);
   }
   uint32_t eos_mark[2] = {0xFFFFFFFFu, 0u};
   append(eos_mark, 8);

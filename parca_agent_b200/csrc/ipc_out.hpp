@@ -150,10 +150,16 @@ class StreamPlan {
  public:
   std::vector<Placement> placements;
   uint64_t total = 0;
+  // One entry per message, in stream order: its encapsulated metadata (continuation marker and padding included) sits at
+  // `at`, its body at `body_at`, and its buffers are placements[p0 .. p1).
+  struct Message { uint64_t at, body_at, body_len; size_t p0, p1; };
+  std::vector<Message> messages;
+  const std::vector<uint8_t>& message_meta(size_t i) const { return meta_[i].second; }
 
   // pass 1: compute the layout. `meta` receives (offset, bytes) blobs to memcpy into the output.
   void build(const std::vector<Node>& columns, const std::vector<std::pair<std::string, std::string>>& schema_md, int64_t n_rows) {
     placements.clear();
+    messages.clear();
     meta_.clear();
     total = 0;
     next_dict_id_ = 0;
@@ -284,6 +290,7 @@ class StreamPlan {
     memcpy(blob.data(), pre, 8);
     memcpy(blob.data() + 8, b.data(), n);
     meta_.push_back({total, std::move(blob)});
+    messages.push_back(Message{total, total + 8 + padded, body.size, placements.size(), placements.size() + body.srcs.size()});
     total += 8 + padded;
     for (size_t i = 0; i < body.srcs.size(); i++) placements.push_back(Placement{body.srcs[i], total + (uint64_t)body.buffers[2 * i]});
     total += body.size;

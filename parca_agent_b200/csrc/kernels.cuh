@@ -2893,4 +2893,168 @@ __global__ void __launch_bounds__(kThreads) k_merge_cols(const EdgeCol* edges /*
   }
 }
 
+// ---------------------------------------------------------------------------------------------
+// LZ4_FRAME body compression on the device (PA_IPC_LZ4_FRAME_GPU). Every non-empty Arrow buffer of the stream becomes one
+// LZ4 frame of independent blocks of at most 64 KiB of input; one warp encodes one block. The encoding is a function of the
+// block's bytes alone (no atomics, no dependence on grid size or timing), and keeps every LZ4 block rule: matches of 4 or
+// more bytes, offsets 1..65535 inside the block, the last match starting 13 or more bytes before the block's end and ending
+// 5 or more bytes before it.
+constexpr uint32_t kLz4Block = 65536;
+constexpr int kLz4HashLog = 12;
+constexpr int kLz4Warps = 4;       // warps per thread block: 4 x 8 KiB hash tables
+constexpr uint16_t kLz4Empty = 0xFFFF;  // no position: a match never starts at 65535 (the last start is len - 13)
+
+struct Lz4Blk { const uint8_t* src; uint32_t len; uint32_t buf; };    // src == nullptr: zeros
+struct Lz4Buf { uint64_t len; uint32_t first, nblk; };                // blocks first .. first+nblk-1 of one Arrow buffer
+
+__device__ __forceinline__ uint32_t lz4_byte(const uint8_t* s, uint32_t i) { return s ? (uint32_t)__ldg(s + i) : 0u; }
+__device__ __forceinline__ uint32_t lz4_word(const uint8_t* s, uint32_t i) {
+  return s ? (uint32_t)__ldg(s + i) | (uint32_t)__ldg(s + i + 1) << 8 | (uint32_t)__ldg(s + i + 2) << 16 | (uint32_t)__ldg(s + i + 3) << 24 : 0u;
+}
+__device__ __forceinline__ uint32_t lz4_hash(uint32_t v) { return (v * 2654435761u) >> (32 - kLz4HashLog); }
+
+// One sequence (nlit literals from src[lit0..], then a match of mlen bytes at distance off; mlen == 0: the closing literals),
+// written by the whole warp at out[*op]. False when it would not fit in `cap` bytes (the block is then stored raw).
+__device__ __forceinline__ bool lz4_sequence(uint8_t* out, uint32_t* op, uint32_t cap, const uint8_t* src, uint32_t lit0, uint32_t nlit,
+                                             uint32_t off, uint32_t mlen, uint32_t lane) {
+  const uint32_t ml = mlen ? mlen - 4 : 0;
+  const uint32_t litx = nlit >= 15 ? (nlit - 15) / 255 + 1 : 0, mlx = ml >= 15 ? (ml - 15) / 255 + 1 : 0;
+  const uint32_t total = 1 + litx + nlit + (mlen ? 2 + mlx : 0);
+  if (*op + total > cap) return false;
+  uint8_t* o = out + *op;
+  if (lane == 0) o[0] = (uint8_t)(min(nlit, 15u) << 4 | min(ml, 15u));
+  for (uint32_t j = lane; j < litx; j += 32) o[1 + j] = j + 1 < litx ? 255 : (uint8_t)((nlit - 15) % 255);
+  for (uint32_t j = lane; j < nlit; j += 32) o[1 + litx + j] = (uint8_t)lz4_byte(src, lit0 + j);
+  if (mlen) {
+    uint8_t* q = o + 1 + litx + nlit;
+    if (lane == 0) { q[0] = (uint8_t)(off & 0xFF); q[1] = (uint8_t)(off >> 8); }
+    for (uint32_t j = lane; j < mlx; j += 32) q[2 + j] = j + 1 < mlx ? 255 : (uint8_t)((ml - 15) % 255);
+  }
+  *op += total;
+  return true;
+}
+
+// Greedy LZ4 of one block per warp. Each step looks up the 32 positions p..p+31 at once in a hash table of block-relative
+// positions; the lowest position whose candidate matches starts the next match, which is extended 32 bytes per ballot. Lanes
+// that share a hash slot insert their positions with a fixed rule (the highest position wins). blk_size[b] = compressed
+// bytes, or 0x80000000 | len when the encoding would not be smaller than the block (stored raw).
+__global__ void __launch_bounds__(kLz4Warps * 32) k_lz4_compress(const Lz4Blk* __restrict__ blks, uint32_t nblk, uint8_t* __restrict__ slots,
+                                                                uint32_t* __restrict__ blk_size) {
+  __shared__ uint16_t tab_all[kLz4Warps][1 << kLz4HashLog];
+  const uint32_t lane = threadIdx.x & 31, b = blockIdx.x * kLz4Warps + (threadIdx.x >> 5);
+  if (b >= nblk) return;  // whole warps only
+  uint16_t* tab = tab_all[threadIdx.x >> 5];
+  const Lz4Blk k = blks[b];
+  const uint8_t* src = k.src;
+  const uint32_t n = k.len, cap = n - 1;
+  uint8_t* out = slots + (size_t)b * kLz4Block;
+  for (uint32_t i = lane; i < (1u << kLz4HashLog); i += 32) tab[i] = kLz4Empty;
+  __syncwarp();
+  const int32_t last_start = (int32_t)n - 13;
+  uint32_t op = 0, anchor = 0, p = 0;
+  bool fits = true;
+  while ((int32_t)p <= last_start) {
+    const uint32_t pos = p + lane;
+    const bool valid = (int32_t)pos <= last_start;
+    uint32_t h = kNull, cand = kLz4Empty;
+    bool ok = false;
+    if (valid) {
+      const uint32_t v = lz4_word(src, pos);
+      h = lz4_hash(v);
+      cand = tab[h];
+      ok = cand != kLz4Empty && lz4_word(src, cand) == v;
+    }
+    const unsigned hit = __ballot_sync(~0u, ok);
+    const uint32_t upto = hit ? __ffs(hit) - 1 : 31;  // positions p..p+upto are inserted
+    const uint32_t key = valid && lane <= upto ? h : kNull;
+    const unsigned same = __match_any_sync(~0u, key);
+    if (key != kNull && 31 - __clz(same) == (int)lane) tab[h] = (uint16_t)pos;
+    __syncwarp();
+    if (!hit) { p += 32; continue; }
+    const uint32_t mpos = p + upto, mcand = __shfl_sync(~0u, cand, upto);
+    const uint32_t maxlen = n - 5 - mpos;  // mpos <= n - 13, so maxlen >= 8
+    uint32_t mlen = 4;
+    for (;;) {
+      const uint32_t i = mlen + lane;
+      const bool stop = i >= maxlen || lz4_byte(src, mpos + i) != lz4_byte(src, mcand + i);
+      const unsigned d = __ballot_sync(~0u, stop);
+      if (d) { mlen += __ffs(d) - 1; break; }
+      mlen += 32;
+    }
+    if (!(fits = lz4_sequence(out, &op, cap, src, anchor, mpos - anchor, mpos - mcand, mlen, lane))) break;
+    p = anchor = mpos + mlen;
+    if (lane == 0) tab[lz4_hash(lz4_word(src, p - 2))] = (uint16_t)(p - 2);
+    __syncwarp();
+  }
+  if (fits) fits = lz4_sequence(out, &op, cap, src, anchor, n - anchor, 0, 0, lane);
+  if (lane == 0) blk_size[b] = fits ? op : (0x80000000u | n);
+}
+
+// One warp per buffer: offset of every block inside its frame (counted from the end of the 7-byte frame header) and the
+// frame's whole size (header + blocks with their 4-byte sizes + EndMark).
+__global__ void __launch_bounds__(kThreads) k_lz4_layout(const Lz4Buf* __restrict__ bufs, uint32_t nbuf, const uint32_t* __restrict__ blk_size,
+                                                         uint64_t* __restrict__ blk_off, uint64_t* __restrict__ frame) {
+  const uint32_t lane = threadIdx.x & 31, w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  if (w >= nbuf) return;
+  const Lz4Buf B = bufs[w];
+  uint64_t run = 0;
+  for (uint32_t i0 = 0; i0 < B.nblk; i0 += 32) {
+    const uint32_t i = i0 + lane;
+    const uint32_t sz = i < B.nblk ? 4 + (blk_size[B.first + i] & 0x7FFFFFFFu) : 0;
+    uint32_t incl = sz;
+    for (int d = 1; d < 32; d <<= 1) {
+      const uint32_t t = __shfl_up_sync(~0u, incl, d);
+      if ((int)lane >= d) incl += t;
+    }
+    if (i < B.nblk) blk_off[B.first + i] = run + incl - sz;
+    run += __shfl_sync(~0u, incl, 31);
+  }
+  if (lane == 0) frame[w] = 7 + run + 4;
+}
+
+__device__ __forceinline__ void lz4_warp_copy(uint8_t* dst, const uint8_t* src, uint32_t n, uint32_t lane) {
+  uint32_t j = lane;
+  for (; j + 96 < n; j += 128) {
+    const uint8_t a = (uint8_t)lz4_byte(src, j), b = (uint8_t)lz4_byte(src, j + 32), c = (uint8_t)lz4_byte(src, j + 64), d = (uint8_t)lz4_byte(src, j + 96);
+    dst[j] = a; dst[j + 32] = b; dst[j + 64] = c; dst[j + 96] = d;
+  }
+  for (; j < n; j += 32) dst[j] = (uint8_t)lz4_byte(src, j);
+}
+
+// One warp per block: writes the block where the compressed body puts it. buf_dst[i] = offset of buffer i in `body` (bit 63:
+// the buffer is stored raw, as -1 and its bytes). The first block of a buffer writes the int64 length prefix and the frame
+// header, the last one the EndMark and the zero padding up to the next 8-byte boundary.
+__global__ void __launch_bounds__(kThreads) k_lz4_pack(const Lz4Blk* __restrict__ blks, uint32_t nblk, const Lz4Buf* __restrict__ bufs,
+                                                       const uint8_t* __restrict__ slots, const uint32_t* __restrict__ blk_size,
+                                                       const uint64_t* __restrict__ blk_off, const uint64_t* __restrict__ frame,
+                                                       const uint64_t* __restrict__ buf_dst, uint8_t* __restrict__ body) {
+  const uint32_t lane = threadIdx.x & 31, b = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  if (b >= nblk) return;
+  const Lz4Blk k = blks[b];
+  const Lz4Buf B = bufs[k.buf];
+  const uint64_t d = buf_dst[k.buf];
+  const bool raw = d >> 63, first = b == B.first, last = b + 1 == B.first + B.nblk;
+  uint8_t* dst = body + (d & ~(1ull << 63));
+  uint64_t end;
+  if (raw) {
+    if (first && lane == 0) *reinterpret_cast<long long*>(dst) = -1;
+    lz4_warp_copy(dst + 8 + (uint64_t)(b - B.first) * kLz4Block, k.src, k.len, lane);
+    end = 8 + B.len;
+  } else {
+    if (first && lane < 15) {  // then the frame header 04 22 4D 18 60 40 82: magic, FLG, BD (64 KiB blocks), HC
+      constexpr uint64_t kHdr = 0x00824060184D2204ull;
+      dst[lane] = (uint8_t)(lane < 8 ? B.len >> (8 * lane) : kHdr >> (8 * (lane - 8)));
+    }
+    const uint32_t sz = blk_size[b], n = sz & 0x7FFFFFFFu;
+    uint8_t* o = dst + 15 + blk_off[b];
+    if (lane < 4) o[lane] = (uint8_t)(sz >> (8 * lane));
+    if (sz >> 31) lz4_warp_copy(o + 4, k.src, n, lane);
+    else lz4_warp_copy(o + 4, slots + (size_t)b * kLz4Block, n, lane);
+    end = 8 + frame[k.buf];
+    if (last && lane < 4) dst[end - 4 + lane] = 0;  // EndMark
+  }
+  if (last)
+    for (uint64_t i = end + lane; i < ((end + 7) & ~7ull); i += 32) dst[i] = 0;
+}
+
 }  // namespace pa

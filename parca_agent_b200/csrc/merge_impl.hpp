@@ -1039,12 +1039,20 @@ static int merge_collect(pa_merge* g, uint8_t* base, uint64_t cap, pa_agg_result
 
 }  // namespace pa
 
+// merged records are never compressed, so a member that asks for device-side LZ4 cannot get it: refused, with the reason in
+// the member's pa_agg_last_error
+static bool lz4_gpu_member(pa_agg* m) {
+  if (!m || m->cfg.ipc_compression != PA_IPC_LZ4_FRAME_GPU) return false;
+  m->fail(PA_EINVAL, "merge groups build uncompressed records: a member created with PA_IPC_LZ4_FRAME_GPU cannot join one");
+  return true;
+}
+
 // ---------------------------------------------------------------------------------------------------------------------
 extern "C" {
 
 int pa_merge_create_local(pa_agg* const* members, uint32_t n, pa_merge** out) {
   if (!members || !n || !out || n > (uint32_t)kMaxWorld) return PA_EINVAL;
-  for (uint32_t i = 0; i < n; i++) if (!members[i] || members[i]->device != members[0]->device) return PA_EINVAL;
+  for (uint32_t i = 0; i < n; i++) if (!members[i] || members[i]->device != members[0]->device || lz4_gpu_member(members[i])) return PA_EINVAL;
   pa_merge* g = new pa_merge();
   g->world = n;
   for (uint32_t i = 0; i < n; i++) { g->members.push_back(members[i]); g->ranks.push_back(i); }
@@ -1063,7 +1071,7 @@ int pa_merge_nccl_unique_id(uint8_t* id128) {
   return PA_OK;
 }
 int pa_merge_create_nccl(pa_agg* member, const uint8_t* id128, uint32_t rank, uint32_t world, pa_merge** out) {
-  if (!member || !id128 || !out || world == 0 || world > (uint32_t)kMaxWorld || rank >= world) return PA_EINVAL;
+  if (!member || !id128 || !out || world == 0 || world > (uint32_t)kMaxWorld || rank >= world || lz4_gpu_member(member)) return PA_EINVAL;
   NcclApi* n = nccl_api();
   if (!n) return PA_EIO;
   if (cudaSetDevice(member->device) != cudaSuccess) return PA_ENODEV;
@@ -1082,7 +1090,8 @@ int pa_merge_create_nccl(pa_agg* member, const uint8_t* id128, uint32_t rank, ui
   return PA_OK;
 }
 int pa_merge_create_host(pa_agg* member, const pa_merge_host_transport* t, uint32_t rank, uint32_t world, pa_merge** out) {
-  if (!member || !t || !out || world == 0 || world > (uint32_t)kMaxWorld || rank >= world || !t->allgather || !t->allgatherv || !t->alltoallv || !t->allreduce_min_u32)
+  if (!member || !t || !out || world == 0 || world > (uint32_t)kMaxWorld || rank >= world || !t->allgather || !t->allgatherv || !t->alltoallv || !t->allreduce_min_u32 ||
+      lz4_gpu_member(member))
     return PA_EINVAL;
   pa_merge* g = new pa_merge();
   g->world = world;
@@ -1096,7 +1105,7 @@ int pa_merge_create_host(pa_agg* member, const pa_merge_host_transport* t, uint3
   return PA_OK;
 }
 int pa_merge_create_shm(pa_agg* member, const char* name, uint32_t rank, uint32_t world, uint64_t mailbox_bytes, pa_merge** out) {
-  if (!member || !name || name[0] != '/' || !out || world == 0 || world > (uint32_t)kMaxWorld || rank >= world) return PA_EINVAL;
+  if (!member || !name || name[0] != '/' || !out || world == 0 || world > (uint32_t)kMaxWorld || rank >= world || lz4_gpu_member(member)) return PA_EINVAL;
   if (mailbox_bytes == 0) mailbox_bytes = 64ull << 20;
   mailbox_bytes = (mailbox_bytes + 4095) & ~4095ull;
   const size_t len = kShmHeaderBytes + (size_t)world * mailbox_bytes;

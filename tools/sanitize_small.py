@@ -2,7 +2,9 @@
 added in round 2 — early copy-out during a multi-chunk flush, the v1 LRU store (evictions, revivals, compaction, over-full batch),
 the pipelined / bulk-copy-staged hash variants, the narrow ring, a 3-shard merged record.
 
-usage: PA_EARLY_D2H_ALWAYS=1 compute-sanitizer --tool memcheck python tools/sanitize_small.py"""
+usage: PA_EARLY_D2H_ALWAYS=1 compute-sanitizer --tool memcheck python tools/sanitize_small.py [plain|lz4_gpu]
+lz4_gpu: small flushes with the bodies compressed on the device (PA_IPC_LZ4_FRAME_GPU) instead: a multi-chunk v2 batch, the
+narrow ring, and a v1 batch with its stacktrace record, each checked against the oracle's plain stream."""
 import os
 import sys
 
@@ -15,8 +17,35 @@ from oracle import oracle_py  # noqa: E402
 from parca_agent_b200 import abi, lib, sharded, synth  # noqa: E402
 
 
+def lz4_gpu():
+    from test_ipc_lz4_gpu import check_stream
+    base = synth.edge_workload(seed=3, n=3000, hash_mode=abi.PA_HASH_XXH64X2)
+    for kw in ({}, {"frame_id_bytes": 4}):
+        a = lib.from_workload(base, chunk_samples=450, ipc_compression=abi.PA_IPC_LZ4_FRAME_GPU, **kw)
+        for n in (3000, 1200):
+            w = base.head(n)
+            lib.load(a, w)
+            check_stream(a.flush().ipc_bytes(), oracle_py.run(w)[0])
+        a.close()
+    w = synth.config2(n=3000, u=800, p=1024)
+    w.schema = abi.PA_SCHEMA_V1
+    o = oracle_py.Oracle(w)
+    o.ingest(w.hdrs, w.frame_ids)
+    want, _ = o.flush()
+    a = lib.from_workload(w, ipc_compression=abi.PA_IPC_LZ4_FRAME_GPU)
+    lib.load(a, w)
+    r = a.flush()
+    check_stream(r.ipc_bytes(), want)
+    ids = a.last_stack_ids(r.n_unique_stacks).tobytes()
+    check_stream(a.stacktraces(ids).ipc_bytes(), o.stacktraces(ids)[0])
+    a.close(); o.close()
+    print("sanitize_small lz4_gpu ok")
+
+
 def main():
     oracle_py.build()
+    if sys.argv[1:] == ["lz4_gpu"]:
+        return lz4_gpu()
     # early copy-out: several intervals through one aggregator, 7 chunks each
     base = synth.edge_workload(seed=3, n=3000, hash_mode=abi.PA_HASH_XXH64X2, external=False)
     for kw in ({}, {"frame_id_bytes": 4}):
