@@ -162,7 +162,11 @@ typedef struct pa_agg_config {
                                   independent 64 KiB LZ4 blocks; only the compressed bodies cross PCIe and no liblz4 is needed. It
                                   decodes to the same record and is NOT byte-identical to the Go writer (nor to mode 1). The mode for
                                   the gRPC path. Both modes apply to every result: v2 and v1 sample records and pa_agg_stacktraces.
-                                  Merge groups never compress: pa_merge_create_* refuse a PA_IPC_LZ4_FRAME_GPU member (PA_EINVAL). */
+                                  Merge groups: when EVERY member is PA_IPC_LZ4_FRAME_GPU the merged record is LZ4_FRAME too, byte
+                                  for byte the stream one such aggregator makes from the concatenated rows (see pa_merge_* below). A
+                                  group that mixes PA_IPC_LZ4_FRAME_GPU members with other members is refused (PA_EINVAL). Groups of
+                                  PA_IPC_PLAIN or PA_IPC_LZ4_FRAME members build uncompressed merged records (the host mode is not
+                                  applied to them; pa_ipc_compress_lz4 can be). */
 } pa_agg_config;
 
 /* Result of one flush; memory is library-owned (pinned host) until pa_agg_release. */
@@ -289,6 +293,15 @@ int pa_agg_stage_device_parts(pa_agg* a, const pa_device_part* parts, uint32_t n
  * least *ipc_len bytes that ALL processes of the group share (e.g. a POSIX shared-memory mapping; it is page-locked on first
  * use); rank 0 adds the dictionaries and the metadata, and gets out->ipc == base. base == NULL: groups whose members all live
  * in this process use a library-owned pinned buffer.
+ * LZ4 groups (every member PA_IPC_LZ4_FRAME_GPU): the record and dictionary batch bodies are LZ4_FRAME-compressed on the members'
+ * GPUs, on each buffer's own 64 KiB block grid, so the stream is byte-identical to one PA_IPC_LZ4_FRAME_GPU aggregator's on the
+ * concatenated rows. pa_merge_plan runs the compression (a block that crosses a shard border is assembled by the shard that holds
+ * its first byte, from the following shards' heads, exchanged once) and returns the COMPRESSED *ipc_len, the same on every
+ * rank; pa_merge_collect packs each member's blocks and copies them to their places, rank 0 adds metadata and framing.
+ * pa_agg_last_kernel_ms(member, "lz4", ...) reports each member's share of the compression kernels, and "lz4_heads" (in
+ * *launches, ms = 0) the bytes of block heads the member sent in the last plan. Mixed groups: pa_merge_create_local refuses
+ * them (the reason goes to the PA_IPC_LZ4_FRAME_GPU members' pa_agg_last_error); groups with one member per process find out
+ * in pa_merge_process, which then fails with PA_EINVAL on every rank before any work.
  *   pa_merge_create_host  : one member per call; the caller supplies the four collectives on HOST buffers (MPI, gloo, sockets ...):
  *                           the library stages device buffers through pinned memory around them. For hosts without NCCL, and for
  *                           exercising the multi-process path on one GPU (two processes may share a device). */

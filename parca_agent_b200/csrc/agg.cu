@@ -245,6 +245,7 @@ struct pa_agg {
   std::vector<std::vector<uint8_t>> hostbufs;  // host-built Arrow buffers of the current result
   std::vector<uint8_t> comp_out;               // PA_IPC_LZ4_FRAME: the re-encoded stream the result points at
   DBuf d_lz4, d_lz4_body;                      // PA_IPC_LZ4_FRAME_GPU: block tables, host-source staging and block slots; compressed bodies
+  uint64_t lz4_head_bytes = 0;                 // merge groups in that mode: bytes of block heads this member sent in the last plan
   cudaEvent_t ev_lz4p0 = nullptr, ev_lz4p1 = nullptr;  // around k_lz4_pack (T_LZ4 covers compress + layout)
   Timer tm[T_COUNT];
   uint32_t launches = 0;
@@ -1867,94 +1868,186 @@ static int early_copy_issue(pa_agg* a) {
   return PA_OK;
 }
 
+// ---- PA_IPC_LZ4_FRAME_GPU, shared by single aggregators (lz4_gpu_stream below) and merge groups (merge_impl.hpp) --------
+// The batch messages of `plan` (message 0 is the schema, copied verbatim): their metadata, and where each message's buffers
+// start in a table of every buffer of messages 1.. in stream order.
+static int lz4_read_messages(pa_agg* a, const StreamPlan& plan, std::vector<BatchMeta>* meta, std::vector<uint32_t>* buf0) {
+  const size_t M = plan.messages.size();
+  meta->assign(M, BatchMeta{});
+  buf0->assign(M, 0);
+  std::string why;
+  uint32_t nbuf = 0;
+  for (size_t m = 1; m < M; m++) {
+    const StreamPlan::Message& g = plan.messages[m];
+    const std::vector<uint8_t>& blob = plan.message_meta(m);
+    if (!read_batch_meta(blob.data() + 8, (uint32_t)blob.size() - 8, &(*meta)[m], &why)) return a->fail(PA_EIO, why.c_str());
+    if ((*meta)[m].buffers.size() != 2 * (g.p1 - g.p0)) return a->fail(PA_EIO, "stream plan and batch metadata disagree");
+    (*buf0)[m] = nbuf;
+    nbuf += (uint32_t)(g.p1 - g.p0);
+  }
+  return PA_OK;
+}
+
+// Host side of a block table: one Lz4Buf per buffer, the blocks it compresses (all of them, or one member's share of a merged
+// buffer). A block's source is device memory, zeros (nullptr), or a place in the staging area, which starts with the host
+// sources (`staged`, uploaded with one copy) and continues with room the caller fills on the device.
+struct Lz4Table {
+  std::vector<Lz4Blk> blks;
+  std::vector<Lz4Buf> bufs;
+  std::vector<uint8_t> staged;
+  uint64_t staging = 0;                                  // staging bytes: staged.size() + device-filled room
+  std::vector<std::pair<size_t, uint64_t>> at_staged;    // (block, offset of its source in the staging area)
+  void buffer(uint64_t len) { bufs.push_back(Lz4Buf{len, (uint32_t)blks.size(), 0}); }
+  void block(const uint8_t* src, uint32_t len) { blks.push_back(Lz4Blk{src, len, (uint32_t)bufs.size() - 1}); bufs.back().nblk++; }
+  void block_staged(uint64_t off, uint32_t len) { at_staged.emplace_back(blks.size(), off); block(nullptr, len); }
+  uint64_t stage_host(const void* p, uint64_t n) {  // offset of the copy in the staging area
+    const uint64_t at = staged.size();
+    staged.insert(staged.end(), (const uint8_t*)p, (const uint8_t*)p + n);
+    staging = std::max<uint64_t>(staging, staged.size());
+    return at;
+  }
+  uint64_t reserve(uint64_t n) { staging = std::max<uint64_t>(staging, staged.size()); const uint64_t at = staging; staging += n; return at; }
+};
+// Its device side, carved out of a->d_lz4: the table, per-block sizes and frame offsets, per-buffer frame sizes and destinations,
+// the staging area, and one 64 KiB slot per block for k_lz4_compress.
+struct Lz4Dev {
+  Lz4Blk* blks = nullptr;
+  Lz4Buf* bufs = nullptr;
+  uint32_t* size = nullptr;
+  uint64_t *off = nullptr, *frame = nullptr, *dst = nullptr;
+  uint8_t *staging = nullptr, *slots = nullptr;
+  size_t nb = 0, nbuf = 0;
+};
+// Sizes a->d_lz4 for `t` and points each staged block at its source. Then lz4_upload, the caller's device-side staging, and
+// lz4_compress.
+static int lz4_alloc(pa_agg* a, Lz4Table& t, Lz4Dev* d) {
+  const size_t nb = t.blks.size(), nbuf = t.bufs.size();
+  auto al = [](size_t v) { return (v + 255) & ~(size_t)255; };
+  const size_t o_bufs = al(nb * sizeof(Lz4Blk)), o_size = o_bufs + al(nbuf * sizeof(Lz4Buf)), o_off = o_size + al(nb * 4), o_frame = o_off + al(nb * 8),
+               o_dst = o_frame + al(nbuf * 8), o_staged = o_dst + al(nbuf * 8), o_slots = o_staged + al(t.staging), bytes = o_slots + nb * kLz4Block;
+  CK(a->d_lz4.ensure(std::max<size_t>(bytes, 256)));
+  uint8_t* p = a->d_lz4.as<uint8_t>();
+  d->blks = (Lz4Blk*)p;
+  d->bufs = (Lz4Buf*)(p + o_bufs);
+  d->size = (uint32_t*)(p + o_size);
+  d->off = (uint64_t*)(p + o_off); d->frame = (uint64_t*)(p + o_frame); d->dst = (uint64_t*)(p + o_dst);
+  d->staging = p + o_staged; d->slots = p + o_slots;
+  d->nb = nb; d->nbuf = nbuf;
+  for (auto& hb : t.at_staged) t.blks[hb.first].src = d->staging + hb.second;
+  return PA_OK;
+}
+// Uploads the table and the host sources.
+static int lz4_upload(pa_agg* a, const Lz4Table& t, const Lz4Dev& d, cudaStream_t s) {
+  if (d.nb) CK(cudaMemcpyAsync(d.blks, t.blks.data(), d.nb * sizeof(Lz4Blk), cudaMemcpyHostToDevice, s));
+  if (d.nbuf) CK(cudaMemcpyAsync(d.bufs, t.bufs.data(), d.nbuf * sizeof(Lz4Buf), cudaMemcpyHostToDevice, s));
+  if (!t.staged.empty()) CK(cudaMemcpyAsync(d.staging, t.staged.data(), t.staged.size(), cudaMemcpyHostToDevice, s));
+  return PA_OK;
+}
+// k_lz4_compress + k_lz4_layout (timed as T_LZ4, which this call resets): per block its compressed size and offset inside its
+// buffer's share of blocks, per buffer 11 + the bytes of those blocks (frame header, blocks with their sizes, EndMark).
+static int lz4_compress(pa_agg* a, const Lz4Dev& d, cudaStream_t s) {
+  Timer& tm = a->tm[T_LZ4];
+  tm.launches = 0;
+  CK(cudaEventRecord(tm.a, s));
+  if (d.nb) { k_lz4_compress<<<(unsigned)((d.nb + kLz4Warps - 1) / kLz4Warps), kLz4Warps * 32, 0, s>>>(d.blks, (uint32_t)d.nb, d.slots, d.size); tm.launches++; }
+  if (d.nbuf) { k_lz4_layout<<<(unsigned)((d.nbuf + kWarps - 1) / kWarps), kThreads, 0, s>>>(d.bufs, (uint32_t)d.nbuf, d.size, d.off, d.frame); tm.launches++; }
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(tm.b, s));
+  return PA_OK;
+}
+
+// Layout of an LZ4_FRAME stream from each buffer's length and whole frame size: a buffer is its int64 length and its frame, or -1
+// and its raw bytes when the frame is not smaller than the buffer.
+struct Lz4Layout {
+  std::vector<std::vector<uint8_t>> metas;  // per message: encapsulated metadata (the schema's verbatim)
+  std::vector<uint64_t> at, body_len;       // per message: offset in the stream, body bytes
+  std::vector<uint64_t> buf_at, buf_size;   // per buffer: offset inside its message's body, bytes (prefix included; 0 = empty)
+  std::vector<uint8_t> raw;                 // per buffer: stored raw
+  uint64_t total = 0;                       // stream bytes, end-of-stream marker included
+  uint64_t body_of(size_t m) const { return at[m] + metas[m].size(); }
+};
+static void lz4_layout(const StreamPlan& plan, const std::vector<BatchMeta>& meta, const std::vector<uint32_t>& buf0, const std::vector<uint64_t>& len,
+                       const std::vector<uint64_t>& frame, Lz4Layout* L) {
+  const size_t M = plan.messages.size();
+  L->metas.assign(M, {});
+  L->at.assign(M, 0); L->body_len.assign(M, 0);
+  L->buf_at.assign(len.size(), 0); L->buf_size.assign(len.size(), 0); L->raw.assign(len.size(), 0);
+  uint64_t total = 0;
+  for (size_t m = 0; m < M; m++) {
+    if (m == 0) {
+      L->metas[m] = plan.message_meta(0);
+    } else {
+      const size_t n = plan.messages[m].p1 - plan.messages[m].p0;
+      std::vector<int64_t> sizes(n), offs;
+      for (size_t i = 0; i < n; i++) {
+        const size_t b = buf0[m] + i;
+        sizes[i] = len[b] ? 8 + (int64_t)std::min<uint64_t>(frame[b], len[b]) : 0;
+        L->buf_size[b] = (uint64_t)sizes[i];
+        L->raw[b] = len[b] && frame[b] >= len[b];
+      }
+      int64_t bl = 0;
+      L->metas[m] = lz4_batch_message(meta[m], sizes, &offs, &bl);
+      for (size_t i = 0; i < n; i++) L->buf_at[buf0[m] + i] = (uint64_t)offs[i];
+      L->body_len[m] = (uint64_t)bl;
+    }
+    L->at[m] = total;
+    total += L->metas[m].size() + L->body_len[m];
+  }
+  L->total = total + 8;
+}
+
 // PA_IPC_LZ4_FRAME_GPU: writes the stream `plan` describes to a->out with every record and dictionary batch body compressed
 // on the device (the framing of ipc_compress_lz4; only the compressed bodies cross PCIe). The host assembles the metadata with
 // the same rewrite as the host mode, from the per-buffer frame sizes. *d2h_ms: the copy-out of the bodies.
 static int lz4_gpu_stream(pa_agg* a, const StreamPlan& plan, cudaStream_t s, uint64_t* out_len, float* d2h_ms) {
   const size_t M = plan.messages.size();
-  std::vector<BatchMeta> meta(M);
-  std::vector<uint32_t> buf0(M, 0);  // first entry of each message's buffers in `bufs`
-  std::vector<Lz4Blk> blks;
-  std::vector<Lz4Buf> bufs;
-  std::vector<uint8_t> staged;                              // HOST sources, uploaded with one copy
-  std::vector<std::pair<size_t, uint64_t>> staged_blk;      // (block, its offset in `staged`)
-  std::string why;
-  for (size_t m = 1; m < M; m++) {  // message 0 is the schema (copied verbatim)
-    const StreamPlan::Message& g = plan.messages[m];
-    const std::vector<uint8_t>& blob = plan.message_meta(m);
-    if (!read_batch_meta(blob.data() + 8, (uint32_t)blob.size() - 8, &meta[m], &why)) return a->fail(PA_EIO, why.c_str());
-    if (meta[m].buffers.size() != 2 * (g.p1 - g.p0)) return a->fail(PA_EIO, "stream plan and batch metadata disagree");
-    buf0[m] = (uint32_t)bufs.size();
-    for (size_t i = g.p0; i < g.p1; i++) {
+  std::vector<BatchMeta> meta;
+  std::vector<uint32_t> buf0;
+  if (int rc = lz4_read_messages(a, plan, &meta, &buf0)) return rc;
+  Lz4Table t;
+  std::vector<uint64_t> len;
+  for (size_t m = 1; m < M; m++)
+    for (size_t i = plan.messages[m].p0; i < plan.messages[m].p1; i++) {
       const BufRef& r = plan.placements[i].src;
       if (r.len && r.kind != BufRef::DEVICE && r.kind != BufRef::HOST && r.kind != BufRef::ZEROS) return a->fail(PA_EINVAL, "buffer without a source");
-      bufs.push_back(Lz4Buf{r.len, (uint32_t)blks.size(), (uint32_t)((r.len + kLz4Block - 1) / kLz4Block)});
+      t.buffer(r.len);
+      len.push_back(r.len);
+      const uint64_t h = r.kind == BufRef::HOST && r.len ? t.stage_host(r.ptr, r.len) : 0;
       for (uint64_t o = 0; o < r.len; o += kLz4Block) {
-        if (r.kind == BufRef::HOST) staged_blk.emplace_back(blks.size(), staged.size() + o);
-        blks.push_back(Lz4Blk{r.kind == BufRef::DEVICE ? (const uint8_t*)r.ptr + o : nullptr, (uint32_t)std::min<uint64_t>(kLz4Block, r.len - o), (uint32_t)bufs.size() - 1});
+        const uint32_t n = (uint32_t)std::min<uint64_t>(kLz4Block, r.len - o);
+        if (r.kind == BufRef::HOST) t.block_staged(h + o, n);
+        else t.block(r.kind == BufRef::DEVICE ? (const uint8_t*)r.ptr + o : nullptr, n);
       }
-      if (r.kind == BufRef::HOST && r.len) staged.insert(staged.end(), (const uint8_t*)r.ptr, (const uint8_t*)r.ptr + r.len);
     }
-  }
-  const size_t nb = blks.size(), nbuf = bufs.size();
-  auto al = [](size_t v) { return (v + 255) & ~(size_t)255; };
-  const size_t o_bufs = al(nb * sizeof(Lz4Blk)), o_size = o_bufs + al(nbuf * sizeof(Lz4Buf)), o_off = o_size + al(nb * 4), o_frame = o_off + al(nb * 8),
-               o_dst = o_frame + al(nbuf * 8), o_staged = o_dst + al(nbuf * 8), o_slots = o_staged + al(staged.size()), bytes = o_slots + nb * kLz4Block;
-  CK(a->d_lz4.ensure(std::max<size_t>(bytes, 256)));
-  uint8_t* d = a->d_lz4.as<uint8_t>();
-  for (auto& hb : staged_blk) blks[hb.first].src = d + o_staged + hb.second;
-  Lz4Blk* d_blks = (Lz4Blk*)d;
-  Lz4Buf* d_bufs = (Lz4Buf*)(d + o_bufs);
-  uint32_t* d_size = (uint32_t*)(d + o_size);
-  uint64_t *d_off = (uint64_t*)(d + o_off), *d_frame = (uint64_t*)(d + o_frame), *d_dst = (uint64_t*)(d + o_dst);
-  if (nb) CK(cudaMemcpyAsync(d_blks, blks.data(), nb * sizeof(Lz4Blk), cudaMemcpyHostToDevice, s));
-  if (nbuf) CK(cudaMemcpyAsync(d_bufs, bufs.data(), nbuf * sizeof(Lz4Buf), cudaMemcpyHostToDevice, s));
-  if (!staged.empty()) CK(cudaMemcpyAsync(d + o_staged, staged.data(), staged.size(), cudaMemcpyHostToDevice, s));
-  Timer& t = a->tm[T_LZ4];
-  t.launches = 0;
-  CK(cudaEventRecord(t.a, s));
-  if (nb) { k_lz4_compress<<<(unsigned)((nb + kLz4Warps - 1) / kLz4Warps), kLz4Warps * 32, 0, s>>>(d_blks, (uint32_t)nb, d + o_slots, d_size); t.launches++; }
-  if (nbuf) { k_lz4_layout<<<(unsigned)((nbuf + kWarps - 1) / kWarps), kThreads, 0, s>>>(d_bufs, (uint32_t)nbuf, d_size, d_off, d_frame); t.launches++; }
-  CK(cudaGetLastError());
-  CK(cudaEventRecord(t.b, s));
+  Lz4Dev d;
+  if (int rc = lz4_alloc(a, t, &d)) return rc;
+  if (int rc = lz4_upload(a, t, d, s)) return rc;
+  if (int rc = lz4_compress(a, d, s)) return rc;
+  Timer& tm = a->tm[T_LZ4];
+  const size_t nb = d.nb, nbuf = d.nbuf;
   std::vector<uint64_t> frame(nbuf);
-  if (nbuf) CK(cudaMemcpyAsync(frame.data(), d_frame, nbuf * 8, cudaMemcpyDeviceToHost, s));
+  if (nbuf) CK(cudaMemcpyAsync(frame.data(), d.frame, nbuf * 8, cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
 
-  // ---- layout: a buffer is its int64 length and its frame, or -1 and its raw bytes when the frame is not smaller
-  std::vector<std::vector<uint8_t>> metas(M);
-  std::vector<uint64_t> body_dev(M, 0), body_len(M, 0), at(M, 0), dst(nbuf, 0);
-  uint64_t dev_total = 0, total = 0;
-  for (size_t m = 0; m < M; m++) {
-    if (m == 0) {
-      metas[m] = plan.message_meta(0);
-    } else {
-      const size_t n = plan.messages[m].p1 - plan.messages[m].p0;
-      std::vector<int64_t> sizes(n), offs;
-      for (size_t i = 0; i < n; i++) {
-        const Lz4Buf& B = bufs[buf0[m] + i];
-        sizes[i] = B.len ? 8 + (int64_t)std::min<uint64_t>(frame[buf0[m] + i], B.len) : 0;
-      }
-      int64_t bl = 0;
-      metas[m] = lz4_batch_message(meta[m], sizes, &offs, &bl);
-      for (size_t i = 0; i < n; i++) {
-        const Lz4Buf& B = bufs[buf0[m] + i];
-        dst[buf0[m] + i] = (dev_total + (uint64_t)offs[i]) | (B.len && frame[buf0[m] + i] >= B.len ? 1ull << 63 : 0);
-      }
-      body_dev[m] = dev_total;
-      body_len[m] = (uint64_t)bl;
-      dev_total += (uint64_t)bl;
+  Lz4Layout L;
+  lz4_layout(plan, meta, buf0, len, frame, &L);
+  std::vector<uint64_t> body_dev(M, 0), dst(nbuf, 0);
+  uint64_t dev_total = 0;
+  for (size_t m = 1; m < M; m++) {
+    for (size_t i = 0; i < plan.messages[m].p1 - plan.messages[m].p0; i++) {
+      const size_t b = buf0[m] + i;
+      dst[b] = (dev_total + L.buf_at[b]) | (L.raw[b] ? 1ull << 63 : 0);
     }
-    at[m] = total;
-    total += metas[m].size() + body_len[m];
+    body_dev[m] = dev_total;
+    dev_total += L.body_len[m];
   }
-  total += 8;
+  const uint64_t total = L.total;
   CK(a->d_lz4_body.ensure(std::max<uint64_t>(dev_total, 256)));
-  if (nbuf) CK(cudaMemcpyAsync(d_dst, dst.data(), nbuf * 8, cudaMemcpyHostToDevice, s));
+  if (nbuf) CK(cudaMemcpyAsync(d.dst, dst.data(), nbuf * 8, cudaMemcpyHostToDevice, s));
   CK(cudaEventRecord(a->ev_lz4p0, s));
   if (nb) {
-    k_lz4_pack<<<(unsigned)((nb + kWarps - 1) / kWarps), kThreads, 0, s>>>(d_blks, (uint32_t)nb, d_bufs, d + o_slots, d_size, d_off, d_frame, d_dst, a->d_lz4_body.as<uint8_t>());
-    t.launches++;
+    k_lz4_pack<<<(unsigned)((nb + kWarps - 1) / kWarps), kThreads, 0, s>>>(d.blks, (uint32_t)nb, d.bufs, d.slots, d.size, d.off, d.frame, d.dst, a->d_lz4_body.as<uint8_t>());
+    tm.launches++;
   }
   CK(cudaGetLastError());
   CK(cudaEventRecord(a->ev_lz4p1, s));
@@ -1969,16 +2062,16 @@ static int lz4_gpu_stream(pa_agg* a, const StreamPlan& plan, cudaStream_t s, uin
   }
   CK(cudaEventRecord(a->ev_d2h0, s));
   for (size_t m = 0; m < M; m++)
-    if (body_len[m]) CK(cudaMemcpyAsync(a->out + at[m] + metas[m].size(), a->d_lz4_body.as<uint8_t>() + body_dev[m], body_len[m], cudaMemcpyDeviceToHost, s));
+    if (L.body_len[m]) CK(cudaMemcpyAsync(a->out + L.body_of(m), a->d_lz4_body.as<uint8_t>() + body_dev[m], L.body_len[m], cudaMemcpyDeviceToHost, s));
   CK(cudaEventRecord(a->ev_d2h1, s));
-  for (size_t m = 0; m < M; m++) memcpy(a->out + at[m], metas[m].data(), metas[m].size());
+  for (size_t m = 0; m < M; m++) memcpy(a->out + L.at[m], L.metas[m].data(), L.metas[m].size());
   const uint32_t eos[2] = {0xFFFFFFFFu, 0u};
   memcpy(a->out + total - 8, eos, 8);
   CK(cudaStreamSynchronize(s));
   float ms = 0, pack = 0;
-  cudaEventElapsedTime(&ms, t.a, t.b);
+  cudaEventElapsedTime(&ms, tm.a, tm.b);
   cudaEventElapsedTime(&pack, a->ev_lz4p0, a->ev_lz4p1);
-  t.ms = (double)ms + pack;
+  tm.ms = (double)ms + pack;
   cudaEventElapsedTime(d2h_ms, a->ev_d2h0, a->ev_d2h1);
   *out_len = total;
   return PA_OK;
@@ -2519,6 +2612,13 @@ int pa_agg_last_kernel_ms(const pa_agg* a, const char* name, double* ms, uint32_
       if (launches) *launches = a->tm[t].launches;
       return PA_OK;
     }
+  // PA_IPC_LZ4_FRAME_GPU merge groups (ms is 0): bytes of this member's parts that went to the owners of blocks crossing a part
+  // border in the last pa_merge_plan
+  if (!strcmp(name, "lz4_heads")) {
+    if (ms) *ms = 0;
+    if (launches) *launches = (uint32_t)std::min<uint64_t>(a->lz4_head_bytes, 0xFFFFFFFFu);
+    return PA_OK;
+  }
   // counters of the v1 stack store since creation (ms is 0): table compactions / eviction rounds
   if (!strcmp(name, "store_compactions") || !strcmp(name, "store_evictions")) {
     if (ms) *ms = 0;

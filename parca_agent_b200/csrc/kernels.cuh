@@ -3057,4 +3057,22 @@ __global__ void __launch_bounds__(kThreads) k_lz4_pack(const Lz4Blk* __restrict_
     for (uint64_t i = end + lane; i < ((end + 7) & ~7ull); i += 32) dst[i] = 0;
 }
 
+// Merge groups: one warp per block of this member's share of the frames. buf_dst[i] = offset of buffer i's share in `body` (bit
+// 63: the buffer is stored raw, and the member copies its part of the buffer as it is). Writes the block's 4-byte size and its
+// bytes at blk_off[b] inside the share; the length prefix, frame header, EndMark and padding are written by the group's root.
+__global__ void __launch_bounds__(kThreads) k_lz4_pack_parts(const Lz4Blk* __restrict__ blks, uint32_t nblk, const uint8_t* __restrict__ slots,
+                                                             const uint32_t* __restrict__ blk_size, const uint64_t* __restrict__ blk_off,
+                                                             const uint64_t* __restrict__ buf_dst, uint8_t* __restrict__ body) {
+  const uint32_t lane = threadIdx.x & 31, b = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  if (b >= nblk) return;
+  const Lz4Blk k = blks[b];
+  const uint64_t d = buf_dst[k.buf];
+  if (d >> 63) return;
+  const uint32_t sz = blk_size[b], n = sz & 0x7FFFFFFFu;
+  uint8_t* o = body + d + blk_off[b];
+  if (lane < 4) o[lane] = (uint8_t)(sz >> (8 * lane));
+  if (sz >> 31) lz4_warp_copy(o + 4, k.src, n, lane);
+  else lz4_warp_copy(o + 4, slots + (size_t)b * kLz4Block, n, lane);
+}
+
 }  // namespace pa

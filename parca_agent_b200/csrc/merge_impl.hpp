@@ -143,6 +143,21 @@ struct pa_merge {
   uint64_t out_cap = 0;
   void* registered = nullptr;                   // caller's shared output buffer, page-locked by us
   uint64_t registered_len = 0;
+  // ---- PA_IPC_LZ4_FRAME_GPU groups (every member in that mode): LZ4_FRAME bodies on the whole buffers' 64 KiB block grid
+  bool lz4 = false;
+  struct Lz4Share {                             // one local member's blocks, from pa_merge_plan to pa_merge_collect
+    Lz4Table t;
+    Lz4Dev d;
+    std::vector<uint64_t> contrib, prefix;      // per buffer: bytes of my blocks (4 + size each); of lower ranks' blocks in front
+    std::vector<const uint8_t*> part;           // per buffer: device source of my part of a sliced buffer (raw fallback)
+    uint64_t send = 0, recv = 0;                // my heads, everybody's heads: offsets in the staging area
+  };
+  std::vector<Lz4Share> lzs;
+  std::vector<uint32_t> lz_msg;                 // per buffer (messages 1.., stream order): its message
+  std::vector<size_t> lz_place;                 // per buffer: its placement
+  std::vector<std::vector<std::pair<uint64_t, uint64_t>>> lz_parts;  // per buffer: [world] (offset, bytes) of each part; empty = root only
+  std::vector<uint64_t> lz_frame;               // per buffer: whole frame bytes
+  Lz4Layout lz;
 
   int fail(int code, const std::string& what) { err = what; return code; }
 };
@@ -160,6 +175,11 @@ namespace pa {
     if (r_ != ncclSuccess) return g->fail(PA_EIO, std::string(#expr) + ": " + nccl_api()->GetErrorString(r_)); \
   } while (0)
 
+// A group builds LZ4_FRAME records when every member was created with PA_IPC_LZ4_FRAME_GPU, plain ones when none was; a group
+// that mixes the two is refused (at creation in one process, in pa_merge_process across processes).
+static bool lz4_gpu_member(const pa_agg* m) { return m->cfg.ipc_compression == PA_IPC_LZ4_FRAME_GPU; }
+static const char kLz4Mixed[] = "a merge group builds LZ4_FRAME records only when every member uses PA_IPC_LZ4_FRAME_GPU, and plain ones when none does: "
+                                "this group mixes PA_IPC_LZ4_FRAME_GPU members with other members";
 static cudaStream_t mstream(pa_merge* g, size_t i) { return g->members[i]->s_comp; }
 // An in-process group on one device runs every member on ONE stream while a merge call is active, so that every copy between
 // members is stream-ordered (NCCL groups keep one stream per member: the collectives order them).
@@ -776,14 +796,14 @@ static int merge_process(pa_merge* g) {
   StreamShare share(g);
   auto restore = [] {};
   // ---- rows of every shard -> global row ranges; registrations must be identical (ids are global)
-  struct Dims { uint64_t n, nf; uint32_t ncols, nlab, n_frames, n_cstr, n_labelsets, n_funcs; };
+  struct Dims { uint64_t n, nf; uint32_t ncols, nlab, n_frames, n_cstr, n_labelsets, n_funcs, lz4; };
   std::vector<const void*> src(L);
   std::vector<uint8_t> hb;
   rc = PA_OK;
   for (size_t i = 0; i < L && !rc; i++) {
     pa_agg* a = g->members[i];
     cudaSetDevice(a->device);
-    Dims d{a->N, a->NF, (uint32_t)a->cols.size(), a->n_label_cols, a->P.n_frames, a->P.n_cstr, a->P.n_labelsets, a->P.n_funcs};
+    Dims d{a->N, a->NF, (uint32_t)a->cols.size(), a->n_label_cols, a->P.n_frames, a->P.n_cstr, a->P.n_labelsets, a->P.n_funcs, g->lz4 ? 1u : 0u};
     if (g->mb[i].gather_scratch.ensure(std::max<size_t>((size_t)(W + 1) * sizeof(Dims), 256)) != cudaSuccess) { rc = g->fail(PA_ENOMEM, "device allocation failed"); break; }
     // staged through the tail of the gather scratch (the head receives the gathered block)
     uint8_t* mine = g->mb[i].gather_scratch.as<uint8_t>() + (size_t)W * sizeof(Dims);
@@ -793,6 +813,8 @@ static int merge_process(pa_merge* g) {
   if (!rc) rc = t_allgather_host(g, src, sizeof(Dims), hb);
   if (rc) { restore(); return rc; }
   const Dims* dims = (const Dims*)hb.data();
+  for (uint32_t r = 0; r < W; r++)  // one member per process: the group's mode is settled here, before any work
+    if (dims[r].lz4 != dims[0].lz4) { restore(); return g->fail(PA_EINVAL, kLz4Mixed); }
   g->n_rows.assign(W, 0); g->nf.assign(W, 0); g->row_base.assign(W + 1, 0);
   g->NT = 0; g->NFT = 0;
   for (uint32_t r = 0; r < W; r++) {
@@ -831,6 +853,8 @@ static int merge_process(pa_merge* g) {
   g->processed = true;
   return PA_OK;
 }
+
+static int merge_plan_lz4(pa_merge* g);
 
 // ---------------------------------------------------------------------------------------------------------------------
 // Output. Every process builds the same plan (all inputs are replicated: merged counters, dictionary orders, run keys of the
@@ -902,9 +926,28 @@ static int merge_plan(pa_merge* g, uint64_t* ipc_len) {
   MergeView mv{g->NT, &g->kind_keys};
   if ((rc = collect_nodes(a0, &mv, g->nodes))) return g->fail(rc, a0->err);
   g->plan.build(g->nodes, {{"parca_write_schema_version", "v2"}}, (int64_t)g->NT);
-  *ipc_len = g->plan.total;
+  if (g->lz4 && (rc = merge_plan_lz4(g))) return rc;
+  *ipc_len = g->lz4 ? g->lz.total : g->plan.total;
   g->planned = true;
   return PA_OK;
+}
+
+// Member i's validity words of label column `col` (host copy of `nwords` words; word 0 is the global word runbase / 32), with its
+// border words completed by the other shards' first / last words: every byte from ceil(runbase / 8) up to
+// ceil((runbase + keep) / 8) is then the merged bitmap's.
+static void complete_valid_words(const pa_merge* g, size_t i, uint32_t col, uint32_t* host, uint32_t nwords) {
+  const uint32_t W = g->world, ncols = g->ncols, me = g->ranks[i];
+  const MergeCol mc = g->cols_all[(size_t)me * ncols + col];
+  const uint64_t gw0 = mc.runbase >> 5;  // global index of my word 0
+  for (uint32_t r = 0; r < W; r++) {
+    if (r == me) continue;
+    const MergeCol o = g->cols_all[(size_t)r * ncols + col];
+    if (!o.keep) continue;
+    const uint64_t ow0 = o.runbase >> 5, ow1 = ((uint64_t)o.runbase + o.keep - 1) >> 5;
+    const uint32_t* ov = g->vwords_all.data() + ((size_t)r * std::max<uint32_t>(ncols, 1) + col) * 2;
+    if (ow0 >= gw0 && ow0 < gw0 + nwords) host[ow0 - gw0] |= ov[0];
+    if (ow1 != ow0 && ow1 >= gw0 && ow1 < gw0 + nwords) host[ow1 - gw0] |= ov[1];
+  }
 }
 
 // part of a sliced buffer that member i holds: device pointer, byte offset inside the buffer, bytes
@@ -930,6 +973,298 @@ static void slice_of(const pa_merge* g, size_t i, uintptr_t tag, const void** pt
   }
 }
 
+// ---- PA_IPC_LZ4_FRAME_GPU groups ----------------------------------------------------------------------------------------
+// The merged stream is, byte for byte, the stream one PA_IPC_LZ4_FRAME_GPU aggregator makes from the concatenated rows: every
+// buffer is cut on ITS 64 KiB block grid, and a block's encoding depends on its bytes alone. Block k of a sliced buffer belongs
+// to the member whose part holds the block's first byte. A block that runs past that part's end needs the heads of the
+// following parts (their bytes up to the next grid boundary); every member publishes its heads in one all-gather, and each owner
+// assembles its crossing blocks in its staging area. The root compresses the replicated, host-built and zero buffers alone. One
+// all-gather of every member's compressed bytes per buffer then gives every rank the same layout, and with it the same ipc_len.
+static int merge_plan_lz4(pa_merge* g) {
+  const size_t L = g->members.size();
+  const uint32_t W = g->world, ncols = g->ncols;
+  const StreamPlan& plan = g->plan;
+  const size_t M = plan.messages.size();
+  pa_agg* a0 = g->members[0];
+  int rc;
+  std::vector<BatchMeta> meta;
+  std::vector<uint32_t> buf0;
+  if ((rc = lz4_read_messages(a0, plan, &meta, &buf0))) return g->fail(rc, a0->err);
+  // ---- every rank's extent of the location-index stream (the other part extents follow from replicated state)
+  std::vector<const void*> csrc(L);
+  for (size_t i = 0; i < L; i++) csrc[i] = g->mb[i].ctl.as<uint32_t>() + CTL_MERGE;
+  std::vector<uint8_t> hc;
+  if ((rc = t_allgather_host(g, csrc, sizeof(MergeCtl), hc))) return rc;
+  const MergeCtl* ctl_all = (const MergeCtl*)hc.data();
+  auto extent = [&](uint32_t r, uintptr_t tag) -> std::pair<uint64_t, uint64_t> {
+    const uint32_t kind = (uint32_t)(tag >> 16), col = (uint32_t)(tag & 0xFFFFu);
+    const uint64_t rb = g->row_base[r], n = g->n_rows[r];
+    switch (kind) {
+      case SL_TS: case SL_VALUE: return {rb * 8, n * 8};
+      case SL_UUID: return {rb * 16, n * 16};
+      case SL_STOFF: case SL_STSIZE: return {rb * 4, n * 4};
+      case SL_STREAM: return {(uint64_t)ctl_all[r].off0 * 4, (uint64_t)ctl_all[r].slice_len * 4};
+      case SL_RUN_ENDS: case SL_RUN_KEYS: { const MergeCol mc = g->cols_all[(size_t)r * ncols + col]; return {(uint64_t)mc.runbase * 4, (uint64_t)mc.keep * 4}; }
+      case SL_VALID: {
+        const MergeCol mc = g->cols_all[(size_t)r * ncols + col];
+        const uint64_t b0 = ((uint64_t)mc.runbase + 7) / 8, b1 = ((uint64_t)mc.runbase + mc.keep + 7) / 8;
+        return {b0, b1 - b0};
+      }
+      default: return {0, 0};
+    }
+  };
+  // ---- buffers, their parts, and the heads every rank publishes (rank r's heads back to back, in buffer order)
+  g->lz_msg.clear(); g->lz_place.clear(); g->lz_parts.clear();
+  std::vector<uint64_t> len;
+  for (size_t m = 1; m < M; m++)
+    for (size_t p = plan.messages[m].p0; p < plan.messages[m].p1; p++) {
+      const BufRef& r = plan.placements[p].src;
+      g->lz_msg.push_back((uint32_t)m); g->lz_place.push_back(p); len.push_back(r.len);
+      g->lz_parts.emplace_back();
+      if (!r.len || r.kind != BufRef::SLICED) continue;
+      auto& parts = g->lz_parts.back();
+      uint64_t pos = 0;
+      for (uint32_t q = 0; q < W; q++) {
+        parts.push_back(extent(q, (uintptr_t)r.ptr));
+        if (!parts.back().second) continue;
+        if (parts.back().first != pos) return g->fail(PA_EIO, "the shards' parts of a merged buffer do not follow each other");
+        pos += parts.back().second;
+      }
+      if (pos != r.len) return g->fail(PA_EIO, "the shards' parts of a merged buffer do not cover it");
+    }
+  const size_t nbuf = len.size();
+  auto head_of = [&](size_t b, uint32_t q) -> uint64_t {  // bytes of part q in front of the first grid boundary inside it
+    if (g->lz_parts[b].empty()) return 0;
+    const auto [at, n] = g->lz_parts[b][q];
+    if (!n || at % kLz4Block == 0) return 0;
+    return std::min<uint64_t>(at + n, (at / kLz4Block + 1) * kLz4Block) - at;
+  };
+  std::vector<std::vector<uint64_t>> head_at(nbuf, std::vector<uint64_t>(W, 0));
+  std::vector<uint64_t> hcount(W, 0), hdispl(W, 0);
+  uint64_t htot = 0;
+  for (uint32_t q = 0; q < W; q++) {
+    for (size_t b = 0; b < nbuf; b++) { head_at[b][q] = hcount[q]; hcount[q] += head_of(b, q); }
+    hdispl[q] = htot;
+    htot += hcount[q];
+  }
+  // ---- per member: validity parts completed on the host, the block table, the staging area
+  struct Copy { const uint8_t* src; int64_t staged_src; uint64_t dst_staged, n; };  // staged_src >= 0: source in the staging area
+  std::vector<std::vector<Copy>> pre(L), post(L);  // before the heads exchange (my heads out), after it (crossing blocks)
+  g->lzs.assign(L, pa_merge::Lz4Share{});
+  for (size_t i = 0; i < L; i++) {
+    pa_agg* a = g->members[i];
+    MCK(cudaSetDevice(a->device));
+    const uint32_t me = g->ranks[i];
+    pa_merge::Lz4Share& sh = g->lzs[i];
+    Lz4Table& t = sh.t;
+    std::vector<const uint8_t*> psrc(nbuf, nullptr);
+    std::vector<int64_t> pstaged(nbuf, -1);
+    std::vector<uint64_t> hoff(nbuf, 0);
+    // host sources first (they open the staging area): validity parts, and the root's host-built buffers
+    for (size_t b = 0; b < nbuf; b++) {
+      const BufRef& r = plan.placements[g->lz_place[b]].src;
+      if (!r.len) continue;
+      if (r.kind == BufRef::HOST && me == 0) hoff[b] = t.stage_host(r.ptr, r.len);
+      if (r.kind != BufRef::SLICED || ((uintptr_t)r.ptr >> 16) != SL_VALID || !g->lz_parts[b][me].second) continue;
+      const uint32_t col = (uint32_t)((uintptr_t)r.ptr & 0xFFFFu);
+      const MergeCol mc = g->cols_all[(size_t)me * ncols + col];
+      const uint32_t nw = (mc.vshift + mc.keep + 31) >> 5;
+      std::vector<uint32_t> words(nw);
+      MCK(cudaMemcpyAsync(words.data(), a->cols[col].validity, (size_t)nw * 4, cudaMemcpyDeviceToHost, a->s_comp));
+      MCK(cudaStreamSynchronize(a->s_comp));
+      complete_valid_words(g, i, col, words.data(), nw);
+      const uint64_t gw0 = mc.runbase >> 5, b0 = g->lz_parts[b][me].first;
+      pstaged[b] = (int64_t)t.stage_host((const uint8_t*)words.data() + (b0 - gw0 * 4), g->lz_parts[b][me].second);
+    }
+    const uint64_t send = sh.send = t.reserve(std::max<uint64_t>(hcount[me], 1)), recv = sh.recv = t.reserve(std::max<uint64_t>(htot, 1));
+    sh.part.assign(nbuf, nullptr);
+    for (size_t b = 0; b < nbuf; b++) {
+      const BufRef& r = plan.placements[g->lz_place[b]].src;
+      t.buffer(r.len);
+      if (!r.len) continue;
+      if (r.kind != BufRef::SLICED) {  // the root's alone
+        if (me != 0) continue;
+        if (r.kind != BufRef::DEVICE && r.kind != BufRef::HOST && r.kind != BufRef::ZEROS) return g->fail(PA_EINVAL, "buffer without a source");
+        for (uint64_t o = 0; o < r.len; o += kLz4Block) {
+          const uint32_t n = (uint32_t)std::min<uint64_t>(kLz4Block, r.len - o);
+          if (r.kind == BufRef::HOST) t.block_staged(hoff[b] + o, n);
+          else t.block(r.kind == BufRef::DEVICE ? (const uint8_t*)r.ptr + o : nullptr, n);
+        }
+        continue;
+      }
+      const auto [at, n] = g->lz_parts[b][me];
+      if (!n) continue;
+      if (pstaged[b] < 0) {
+        const void* ptr; uint64_t at2, n2;
+        slice_of(g, i, (uintptr_t)r.ptr, &ptr, &at2, &n2);
+        if (at2 != at || n2 != n) return g->fail(PA_EIO, "a shard's part of a merged buffer changed between its exchange and its use");
+        psrc[b] = (const uint8_t*)ptr;
+      }
+      if (const uint64_t h = head_of(b, me)) pre[i].push_back(Copy{psrc[b], pstaged[b], send + head_at[b][me], h});
+      for (uint64_t k = (at + kLz4Block - 1) / kLz4Block; k * kLz4Block < at + n; k++) {
+        const uint64_t s0 = k * kLz4Block, e = std::min<uint64_t>(s0 + kLz4Block, r.len);
+        if (e <= at + n) {  // inside my part
+          if (pstaged[b] >= 0) t.block_staged((uint64_t)pstaged[b] + (s0 - at), (uint32_t)(e - s0));
+          else t.block(psrc[b] + (s0 - at), (uint32_t)(e - s0));
+          continue;
+        }
+        // crossing block: my tail, then the heads of the parts that start before its end
+        const uint64_t off = t.reserve(e - s0);
+        t.block_staged(off, (uint32_t)(e - s0));
+        post[i].push_back(Copy{pstaged[b] >= 0 ? nullptr : psrc[b] + (s0 - at), pstaged[b] >= 0 ? pstaged[b] + (int64_t)(s0 - at) : -1, off, at + n - s0});
+        for (uint32_t q = me + 1; q < W; q++) {
+          const auto [qat, qn] = g->lz_parts[b][q];
+          if (!qn || qat >= e) continue;
+          post[i].push_back(Copy{nullptr, (int64_t)(recv + hdispl[q] + head_at[b][q]), off + (qat - s0), head_of(b, q)});
+        }
+      }
+    }
+    if ((rc = lz4_alloc(a, t, &sh.d))) return g->fail(rc, a->err);
+    if ((rc = lz4_upload(a, t, sh.d, a->s_comp))) return g->fail(rc, a->err);
+    for (size_t b = 0; b < nbuf; b++) sh.part[b] = pstaged[b] >= 0 ? sh.d.staging + pstaged[b] : psrc[b];
+    for (const Copy& c : pre[i])
+      MCK(cudaMemcpyAsync(sh.d.staging + c.dst_staged, c.staged_src >= 0 ? sh.d.staging + c.staged_src : c.src, c.n, cudaMemcpyDeviceToDevice, a->s_comp));
+    a->lz4_head_bytes = hcount[me];
+  }
+  // ---- the heads exchange
+  if (htot) {
+    std::vector<const void*> hs(L);
+    std::vector<void*> hd(L);
+    for (size_t i = 0; i < L; i++) { hs[i] = g->lzs[i].d.staging + g->lzs[i].send; hd[i] = g->lzs[i].d.staging + g->lzs[i].recv; }
+    if ((rc = t_allgatherv(g, hs, hd, hcount, hdispl))) return rc;
+  }
+  // ---- crossing blocks, compression, and every rank's compressed bytes per buffer
+  std::vector<const void*> fsrc(L);
+  for (size_t i = 0; i < L; i++) {
+    pa_agg* a = g->members[i];
+    MCK(cudaSetDevice(a->device));
+    pa_merge::Lz4Share& sh = g->lzs[i];
+    for (const Copy& c : post[i])
+      MCK(cudaMemcpyAsync(sh.d.staging + c.dst_staged, c.staged_src >= 0 ? sh.d.staging + c.staged_src : c.src, c.n, cudaMemcpyDeviceToDevice, a->s_comp));
+    if ((rc = lz4_compress(a, sh.d, a->s_comp))) return g->fail(rc, a->err);
+    fsrc[i] = sh.d.frame;
+  }
+  std::vector<uint8_t> hf;
+  if (nbuf && (rc = t_allgather_host(g, fsrc, nbuf * 8, hf))) return rc;
+  const uint64_t* fr = (const uint64_t*)hf.data();  // [rank][buffer]: 11 + that rank's bytes of the buffer's blocks
+  g->lz_frame.assign(nbuf, 11);
+  for (size_t i = 0; i < L; i++) { g->lzs[i].contrib.assign(nbuf, 0); g->lzs[i].prefix.assign(nbuf, 0); }
+  for (size_t b = 0; b < nbuf; b++)
+    for (uint32_t q = 0; q < W; q++) {
+      const uint64_t c = fr[(size_t)q * nbuf + b] - 11;
+      for (size_t i = 0; i < L; i++) {
+        if (g->ranks[i] == q) g->lzs[i].contrib[b] = c;
+        if (g->ranks[i] > q) g->lzs[i].prefix[b] += c;
+      }
+      g->lz_frame[b] += c;
+    }
+  lz4_layout(plan, meta, buf0, len, g->lz_frame, &g->lz);
+  return PA_OK;
+}
+
+
+// PA_IPC_LZ4_FRAME_GPU groups: every member packs its blocks and copies each share of a frame to its place in `base` (or, for a
+// buffer stored raw, its part of the buffer); the root writes the metadata, length prefixes, frame headers, EndMarks, padding,
+// the buffers it alone holds when they are stored raw, and the end-of-stream marker. *d2h: the longest member's copy-out.
+static int merge_collect_lz4(pa_merge* g, uint8_t* base, bool root, float* d2h) {
+  const size_t L = g->members.size(), nbuf = g->lz_frame.size();
+  const Lz4Layout& lz = g->lz;
+  const StreamPlan& plan = g->plan;
+  auto buf_at = [&](size_t b) { return lz.body_of(g->lz_msg[b]) + lz.buf_at[b]; };  // its length prefix, in the stream
+  for (size_t i = 0; i < L; i++) {
+    pa_agg* a = g->members[i];
+    MCK(cudaSetDevice(a->device));
+    cudaStream_t s = a->s_comp;
+    pa_merge::Lz4Share& sh = g->lzs[i];
+    const uint32_t me = g->ranks[i];
+    std::vector<uint64_t> dst(nbuf, 0);
+    uint64_t seg = 0;
+    for (size_t b = 0; b < nbuf; b++) {
+      if (lz.raw[b]) { dst[b] = 1ull << 63; continue; }
+      dst[b] = seg;
+      seg += sh.contrib[b];
+    }
+    MCK(a->d_lz4_body.ensure(std::max<uint64_t>(seg, 256)));
+    if (nbuf) MCK(cudaMemcpyAsync(sh.d.dst, dst.data(), nbuf * 8, cudaMemcpyHostToDevice, s));
+    MCK(cudaEventRecord(a->ev_lz4p0, s));
+    if (sh.d.nb) {
+      k_lz4_pack_parts<<<(unsigned)((sh.d.nb + kWarps - 1) / kWarps), kThreads, 0, s>>>(sh.d.blks, (uint32_t)sh.d.nb, sh.d.slots, sh.d.size, sh.d.off, sh.d.dst,
+                                                                                       a->d_lz4_body.as<uint8_t>());
+      a->tm[T_LZ4].launches++;
+    }
+    MCK(cudaGetLastError());
+    MCK(cudaEventRecord(a->ev_lz4p1, s));
+    MCK(cudaEventRecord(a->ev_d2h0, s));
+    for (size_t b = 0; b < nbuf; b++) {
+      const BufRef& r = plan.placements[g->lz_place[b]].src;
+      if (!r.len) continue;
+      if (!lz.raw[b]) {
+        if (sh.contrib[b]) MCK(cudaMemcpyAsync(base + buf_at(b) + 8 + 7 + sh.prefix[b], a->d_lz4_body.as<uint8_t>() + dst[b], sh.contrib[b], cudaMemcpyDeviceToHost, s));
+      } else if (r.kind == BufRef::SLICED) {
+        const auto [at, n] = g->lz_parts[b][me];
+        if (n) MCK(cudaMemcpyAsync(base + buf_at(b) + 8 + at, sh.part[b], n, cudaMemcpyDeviceToHost, s));
+      } else if (r.kind == BufRef::DEVICE && me == 0) {
+        MCK(cudaMemcpyAsync(base + buf_at(b) + 8, r.ptr, r.len, cudaMemcpyDeviceToHost, s));
+      }
+    }
+    MCK(cudaEventRecord(a->ev_d2h1, s));
+  }
+  if (root) {  // overlaps the copies: none of these bytes is written by a member
+    for (size_t m = 0; m < lz.metas.size(); m++) memcpy(base + lz.at[m], lz.metas[m].data(), lz.metas[m].size());
+    static const uint8_t kHdr[7] = {0x04, 0x22, 0x4D, 0x18, 0x60, 0x40, 0x82};
+    for (size_t b = 0; b < nbuf; b++) {
+      const BufRef& r = plan.placements[g->lz_place[b]].src;
+      if (!r.len) continue;
+      uint8_t* o = base + buf_at(b);
+      const int64_t prefix = lz.raw[b] ? -1 : (int64_t)r.len;
+      memcpy(o, &prefix, 8);
+      if (!lz.raw[b]) {
+        memcpy(o + 8, kHdr, 7);
+        memset(o + 8 + g->lz_frame[b] - 4, 0, 4);  // EndMark
+      } else if (r.kind == BufRef::HOST) {
+        memcpy(o + 8, r.ptr, r.len);
+      } else if (r.kind == BufRef::ZEROS) {
+        memset(o + 8, 0, r.len);
+      }
+      const uint64_t n = lz.buf_size[b];
+      memset(o + n, 0, ((n + 7) & ~7ull) - n);
+    }
+    const uint32_t eos[2] = {0xFFFFFFFFu, 0u};
+    memcpy(base + lz.total - 8, eos, 8);
+  }
+  int rc = msync(g);
+  if (rc) return rc;
+  *d2h = 0;
+  for (size_t i = 0; i < L; i++) {
+    pa_agg* a = g->members[i];
+    float ms = 0, pack = 0, copy = 0;
+    cudaEventElapsedTime(&ms, a->tm[T_LZ4].a, a->tm[T_LZ4].b);
+    cudaEventElapsedTime(&pack, a->ev_lz4p0, a->ev_lz4p1);
+    cudaEventElapsedTime(&copy, a->ev_d2h0, a->ev_d2h1);
+    a->tm[T_LZ4].ms = (double)ms + pack;
+    *d2h = std::max(*d2h, copy);
+  }
+  return PA_OK;
+}
+
+template <class Done>
+static int merge_result(pa_merge* g, uint8_t* base, bool root, uint64_t total, double t0, float d2h, pa_agg_result* res, Done& done) {
+  const double t1 = now_ms();
+  const size_t L = g->members.size();
+  pa_agg* a0 = g->members[0];
+  const Counters& c = a0->h_ctr;
+  res->ipc = root ? base : nullptr; res->ipc_len = total; res->n_rows = g->NT; res->n_unique_stacks = c.n_unique; res->n_locations = c.n_locations;
+  res->n_functions = c.n_functions; res->n_location_indices = (uint32_t)c.n_indices64;
+  res->gpu_launches = 0;
+  for (size_t i = 0; i < L; i++) res->gpu_launches += g->members[i]->launches;
+  res->gpu_ms = a0->tm[T_TOTAL].ms; res->d2h_ms = d2h; res->host_ms = std::max(0.0, (t1 - t0) - d2h);
+  float h2d = 0;
+  cudaEventElapsedTime(&h2d, a0->ev_h2d0, a0->ev_h2d1);
+  res->h2d_ms = h2d;
+  done();
+  return PA_OK;
+}
+
 static int merge_collect(pa_merge* g, uint8_t* base, uint64_t cap, pa_agg_result* res) {
   memset(res, 0, sizeof *res);
   if (!g->planned) return g->fail(PA_EINVAL, "pa_merge_collect before pa_merge_plan");
@@ -938,7 +1273,7 @@ static int merge_collect(pa_merge* g, uint8_t* base, uint64_t cap, pa_agg_result
   auto done = [&] { for (size_t i = 0; i < L; i++) { release_staged(g->members[i]); g->members[i]->merged_part = false; } g->planned = false; g->processed = false; };
   if (g->NT == 0) { done(); return PA_OK; }
   const double t0 = now_ms();
-  const uint64_t total = g->plan.total;
+  const uint64_t total = g->lz4 ? g->lz.total : g->plan.total;
   StreamShare share(g);
   bool root = false;
   for (size_t i = 0; i < L; i++) root |= g->ranks[i] == 0;
@@ -960,6 +1295,11 @@ static int merge_collect(pa_merge* g, uint8_t* base, uint64_t cap, pa_agg_result
       if (cudaHostRegister(base, cap, cudaHostRegisterPortable) == cudaSuccess) { g->registered = base; g->registered_len = cap; }
       else cudaGetLastError();  // not fatal: pageable copies are slower but correct
     }
+  }
+  float d2h = 0;
+  if (g->lz4) {
+    if (int rc = merge_collect_lz4(g, base, root, &d2h)) return rc;
+    return merge_result(g, base, root, total, t0, d2h, res, done);
   }
   // ---- device -> host: every member its parts; the root also the replicated buffers
   struct BitJob { size_t member; uint32_t col; uint64_t at; uint32_t* host; uint32_t nwords; };
@@ -1008,53 +1348,34 @@ static int merge_collect(pa_merge* g, uint8_t* base, uint64_t cap, pa_agg_result
     const uint32_t me = g->ranks[b.member];
     const MergeCol mc = g->cols_all[(size_t)me * ncols + b.col];
     const uint64_t gw0 = mc.runbase >> 5;  // global index of my word 0
-    for (uint32_t r = 0; r < W; r++) {
-      if (r == me) continue;
-      const MergeCol o = g->cols_all[(size_t)r * ncols + b.col];
-      if (!o.keep) continue;
-      const uint64_t ow0 = o.runbase >> 5, ow1 = ((uint64_t)o.runbase + o.keep - 1) >> 5;
-      const uint32_t* ov = g->vwords_all.data() + ((size_t)r * std::max<uint32_t>(ncols, 1) + b.col) * 2;
-      if (ow0 >= gw0 && ow0 < gw0 + b.nwords) b.host[ow0 - gw0] |= ov[0];
-      if (ow1 != ow0 && ow1 >= gw0 && ow1 < gw0 + b.nwords) b.host[ow1 - gw0] |= ov[1];
-    }
+    complete_valid_words(g, b.member, b.col, b.host, b.nwords);
     const uint64_t b0 = ((uint64_t)mc.runbase + 7) / 8, b1 = ((uint64_t)mc.runbase + mc.keep + 7) / 8;
     if (b1 > b0) memcpy(base + b.at + b0, (const uint8_t*)b.host + (b0 - gw0 * 4), b1 - b0);
   }
-  const double t1 = now_ms();
-  float d2h = 0;
   for (size_t i = 0; i < L; i++) { float ms = 0; cudaEventElapsedTime(&ms, g->members[i]->ev_d2h0, g->members[i]->ev_d2h1); d2h = std::max(d2h, ms); }
-  pa_agg* a0 = g->members[0];
-  const Counters& c = a0->h_ctr;
-  res->ipc = root ? base : nullptr; res->ipc_len = total; res->n_rows = g->NT; res->n_unique_stacks = c.n_unique; res->n_locations = c.n_locations;
-  res->n_functions = c.n_functions; res->n_location_indices = (uint32_t)c.n_indices64;
-  res->gpu_launches = 0;
-  for (size_t i = 0; i < L; i++) res->gpu_launches += g->members[i]->launches;
-  res->gpu_ms = a0->tm[T_TOTAL].ms; res->d2h_ms = d2h; res->host_ms = std::max(0.0, (t1 - t0) - d2h);
-  float h2d = 0;
-  cudaEventElapsedTime(&h2d, a0->ev_h2d0, a0->ev_h2d1);
-  res->h2d_ms = h2d;
-  done();
-  return PA_OK;
+  return merge_result(g, base, root, total, t0, d2h, res, done);
 }
 
 }  // namespace pa
 
-// merged records are never compressed, so a member that asks for device-side LZ4 cannot get it: refused, with the reason in
-// the member's pa_agg_last_error
-static bool lz4_gpu_member(pa_agg* m) {
-  if (!m || m->cfg.ipc_compression != PA_IPC_LZ4_FRAME_GPU) return false;
-  m->fail(PA_EINVAL, "merge groups build uncompressed records: a member created with PA_IPC_LZ4_FRAME_GPU cannot join one");
-  return true;
-}
 
 // ---------------------------------------------------------------------------------------------------------------------
 extern "C" {
 
 int pa_merge_create_local(pa_agg* const* members, uint32_t n, pa_merge** out) {
   if (!members || !n || !out || n > (uint32_t)kMaxWorld) return PA_EINVAL;
-  for (uint32_t i = 0; i < n; i++) if (!members[i] || members[i]->device != members[0]->device || lz4_gpu_member(members[i])) return PA_EINVAL;
+  uint32_t n_lz4 = 0;
+  for (uint32_t i = 0; i < n; i++) {
+    if (!members[i] || members[i]->device != members[0]->device) return PA_EINVAL;
+    n_lz4 += lz4_gpu_member(members[i]);
+  }
+  if (n_lz4 && n_lz4 != n) {  // the reason goes where the caller of a PA_IPC_LZ4_FRAME_GPU member looks for it
+    for (uint32_t i = 0; i < n; i++) if (lz4_gpu_member(members[i])) members[i]->fail(PA_EINVAL, kLz4Mixed);
+    return PA_EINVAL;
+  }
   pa_merge* g = new pa_merge();
   g->world = n;
+  g->lz4 = n_lz4 == n;
   for (uint32_t i = 0; i < n; i++) { g->members.push_back(members[i]); g->ranks.push_back(i); }
   g->mb.resize(n);
   *out = g;
@@ -1071,7 +1392,7 @@ int pa_merge_nccl_unique_id(uint8_t* id128) {
   return PA_OK;
 }
 int pa_merge_create_nccl(pa_agg* member, const uint8_t* id128, uint32_t rank, uint32_t world, pa_merge** out) {
-  if (!member || !id128 || !out || world == 0 || world > (uint32_t)kMaxWorld || rank >= world || lz4_gpu_member(member)) return PA_EINVAL;
+  if (!member || !id128 || !out || world == 0 || world > (uint32_t)kMaxWorld || rank >= world) return PA_EINVAL;
   NcclApi* n = nccl_api();
   if (!n) return PA_EIO;
   if (cudaSetDevice(member->device) != cudaSuccess) return PA_ENODEV;
@@ -1082,6 +1403,7 @@ int pa_merge_create_nccl(pa_agg* member, const uint8_t* id128, uint32_t rank, ui
   pa_merge* g = new pa_merge();
   g->world = world;
   g->use_nccl = true;
+  g->lz4 = lz4_gpu_member(member);
   g->members.push_back(member);
   g->ranks.push_back(rank);
   g->comms.push_back(comm);
@@ -1090,14 +1412,14 @@ int pa_merge_create_nccl(pa_agg* member, const uint8_t* id128, uint32_t rank, ui
   return PA_OK;
 }
 int pa_merge_create_host(pa_agg* member, const pa_merge_host_transport* t, uint32_t rank, uint32_t world, pa_merge** out) {
-  if (!member || !t || !out || world == 0 || world > (uint32_t)kMaxWorld || rank >= world || !t->allgather || !t->allgatherv || !t->alltoallv || !t->allreduce_min_u32 ||
-      lz4_gpu_member(member))
+  if (!member || !t || !out || world == 0 || world > (uint32_t)kMaxWorld || rank >= world || !t->allgather || !t->allgatherv || !t->alltoallv || !t->allreduce_min_u32)
     return PA_EINVAL;
   pa_merge* g = new pa_merge();
   g->world = world;
   g->use_nccl = true;  // one stream per member; ordering comes from the (synchronous) collectives
   g->host_copy = *t;
   g->host = &g->host_copy;
+  g->lz4 = lz4_gpu_member(member);
   g->members.push_back(member);
   g->ranks.push_back(rank);
   g->mb.resize(1);
@@ -1105,7 +1427,7 @@ int pa_merge_create_host(pa_agg* member, const pa_merge_host_transport* t, uint3
   return PA_OK;
 }
 int pa_merge_create_shm(pa_agg* member, const char* name, uint32_t rank, uint32_t world, uint64_t mailbox_bytes, pa_merge** out) {
-  if (!member || !name || name[0] != '/' || !out || world == 0 || world > (uint32_t)kMaxWorld || rank >= world || lz4_gpu_member(member)) return PA_EINVAL;
+  if (!member || !name || name[0] != '/' || !out || world == 0 || world > (uint32_t)kMaxWorld || rank >= world) return PA_EINVAL;
   if (mailbox_bytes == 0) mailbox_bytes = 64ull << 20;
   mailbox_bytes = (mailbox_bytes + 4095) & ~4095ull;
   const size_t len = kShmHeaderBytes + (size_t)world * mailbox_bytes;
@@ -1146,6 +1468,7 @@ int pa_merge_create_shm(pa_agg* member, const char* name, uint32_t rank, uint32_
   g->shm_len = len;
   g->shm_name = name;
   g->shm_owner = rank == 0;
+  g->lz4 = lz4_gpu_member(member);
   cudaSetDevice(member->device);
   if (cudaHostRegister(base, len, cudaHostRegisterPortable) == cudaSuccess) g->shm_registered = true;  // DMA straight into / out of the mailboxes
   else cudaGetLastError();

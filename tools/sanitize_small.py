@@ -2,9 +2,11 @@
 added in round 2 — early copy-out during a multi-chunk flush, the v1 LRU store (evictions, revivals, compaction, over-full batch),
 the pipelined / bulk-copy-staged hash variants, the narrow ring, a 3-shard merged record.
 
-usage: PA_EARLY_D2H_ALWAYS=1 compute-sanitizer --tool memcheck python tools/sanitize_small.py [plain|lz4_gpu]
+usage: PA_EARLY_D2H_ALWAYS=1 compute-sanitizer --tool memcheck python tools/sanitize_small.py [plain|lz4_gpu|merge_lz4_gpu]
 lz4_gpu: small flushes with the bodies compressed on the device (PA_IPC_LZ4_FRAME_GPU) instead: a multi-chunk v2 batch, the
-narrow ring, and a v1 batch with its stacktrace record, each checked against the oracle's plain stream."""
+narrow ring, and a v1 batch with its stacktrace record, each checked against the oracle's plain stream.
+merge_lz4_gpu: a small in-process merge group of PA_IPC_LZ4_FRAME_GPU members whose shard cuts put blocks across part borders
+(heads exchange, crossing blocks, an empty shard), checked against one such aggregator on the concatenated rows."""
 import os
 import sys
 
@@ -42,10 +44,33 @@ def lz4_gpu():
     print("sanitize_small lz4_gpu ok")
 
 
+def merge_lz4_gpu():
+    from test_ipc_lz4_gpu import check_buffers
+    lz4 = abi.PA_IPC_LZ4_FRAME_GPU
+    w = synth.config1().head(24_000)
+    cuts = [0, 8191, 8191, 8200, 16384, 24_000]
+    idx = [np.arange(cuts[i], cuts[i + 1]) for i in range(len(cuts) - 1)]
+    parts = [w.rows(ix) for ix in idx]
+    aggs = [lib.from_workload(p, ipc_compression=lz4) for p in parts]
+    g = lib.MergeGroup.local(aggs)
+    for _ in range(2):
+        for a, p in zip(aggs, parts):
+            lib.load(a, p)
+        got = g.flush().ipc_bytes()
+        assert got == lib.run(w, ipc_compression=lz4)[0]
+        check_buffers(got, oracle_py.run(w)[0])
+    g.close()
+    for a in aggs:
+        a.close()
+    print("sanitize_small merge_lz4_gpu ok")
+
+
 def main():
     oracle_py.build()
     if sys.argv[1:] == ["lz4_gpu"]:
         return lz4_gpu()
+    if sys.argv[1:] == ["merge_lz4_gpu"]:
+        return merge_lz4_gpu()
     # early copy-out: several intervals through one aggregator, 7 chunks each
     base = synth.edge_workload(seed=3, n=3000, hash_mode=abi.PA_HASH_XXH64X2, external=False)
     for kw in ({}, {"frame_id_bytes": 4}):
