@@ -279,7 +279,7 @@ typedef struct pa_device_part {
 int pa_agg_stage_device_parts(pa_agg* a, const pa_device_part* parts, uint32_t n_parts, uint64_t n_rows_total);
 
 /* ---- multi-GPU, one merged batch with an O(unique keys) exchange (SURVEY section 8e; "mode B, slices") ------------------
- * A group of shard aggregators (PA_SCHEMA_V2, identical string / frame / labelset registrations, one per GPU ring) builds
+ * A group of shard aggregators (one schema, identical string / frame / labelset registrations, one per GPU ring) builds
  * ONE record batch: the reference's record (reporter/parca_reporter.go:1742-1790) for the sample stream
  * [shard 0's rows, shard 1's rows, ...]. Rows never leave the GPU that ingested them; only dictionary keys cross NVLink
  * (stack ids to their owner shard and back as one merged list, min-reductions of the first-occurrence tables, thread-id lists,
@@ -302,6 +302,17 @@ int pa_agg_stage_device_parts(pa_agg* a, const pa_device_part* parts, uint32_t n
  * *launches, ms = 0) the bytes of block heads the member sent in the last plan. Mixed groups: pa_merge_create_local refuses
  * them (the reason goes to the PA_IPC_LZ4_FRAME_GPU members' pa_agg_last_error); groups with one member per process find out
  * in pa_merge_process, which then fails with PA_EINVAL on every rank before any work.
+ * v1 groups (every member PA_SCHEMA_V1, with equal store sizes: stack_cache_entries / stack_cache_frames as they resolve — left
+ * at 0 they follow max_samples, so members with different rings need explicit, equal values): the group behaves, interval by
+ * interval, like ONE v1 aggregator fed the concatenated rows — the sample record, pa_agg_stacktraces, pa_agg_last_stack_ids and
+ * the "store_evictions" / "store_compactions" counters. Every member holds a full copy of the group's known-stacks store and
+ * pa_merge_process applies the merged batch's accesses to each copy (it exchanges the global last row of every merged stack and
+ * the frames of the stacks the store lacks; pa_agg_last_kernel_ms(member, "store_frames", ...) reports, in *launches, the frame
+ * ids the member sent in the last pa_merge_process). An error any member's store update finds (e.g. an unregistered frame id,
+ * seen only by the shard that sends that stack's frames) fails pa_merge_process on every rank. After a merged interval pa_agg_last_stack_ids on any member returns the merged dictionary, and a member
+ * flushed on its own continues from the group's store. A group that mixes schemas, or v1 members with different store sizes, is
+ * refused like a mixed LZ4 group (pa_merge_create_local at once, with the reason in every member's pa_agg_last_error;
+ * multi-process groups in pa_merge_process on every rank).
  *   pa_merge_create_host  : one member per call; the caller supplies the four collectives on HOST buffers (MPI, gloo, sockets ...):
  *                           the library stages device buffers through pinned memory around them. For hosts without NCCL, and for
  *                           exercising the multi-process path on one GPU (two processes may share a device). */
@@ -333,6 +344,13 @@ int pa_merge_plan(pa_merge* m, uint64_t* ipc_len);
 int pa_merge_collect(pa_merge* m, uint8_t* base, uint64_t cap, pa_agg_result* out);
 /* in-process groups: ring swap + H2D of every member, the merged pass, plan and collect in one call */
 int pa_merge_flush(pa_merge* m, pa_agg_result* out);
+/* v1 groups, between intervals (collective): the stacktrace record (pa_agg_stacktraces) for rank 0's request. Rank 0 passes the
+ * server's ids, the other ranks NULL / 0 (the ids reach them in one all-gather). Every member applies the request's accesses to
+ * its copy of the store, and each rank's *out is the record its own member built: the same bytes on every rank (in-process
+ * groups: member 0's). The result is that member's, as if it came from pa_agg_stacktraces on it: out->ipc lives in the member's
+ * pinned output buffer, is replaced by its next flush / collect / stacktrace request, and is released with
+ * pa_agg_release(member, out). PA_EINVAL for v2 groups, and before the merged batch is collected. */
+int pa_merge_stacktraces(pa_merge* m, const uint8_t* ids, uint64_t n_ids, pa_agg_result* out);
 /* wall-clock of the last pa_merge_process, the part of it spent waiting in the three size exchanges, the payload bytes this
  * process's members sent to other ranks (NCCL groups), and the merged row count */
 int pa_merge_last_stats(const pa_merge* m, double* wall_ms, double* exchange_wait_ms, uint64_t* nvlink_bytes, uint64_t* n_rows_total);

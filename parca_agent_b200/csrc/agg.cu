@@ -114,8 +114,9 @@ struct Pass {
   size_t Pn = 1, S = 1, FN = 1, NI = 1;
   size_t cls_bytes[3] = {0, 0, 0};
   uint32_t *rowbits = nullptr, *row_wprefix = nullptr, *uniq_slot = nullptr, *uniq_size = nullptr, *first_ls = nullptr, *claimed = nullptr;
-  uint32_t *loc_bits = nullptr, *loc_wp = nullptr, *sd_bits[4] = {}, *sd_wp[4] = {}, *fn_bits = nullptr, *fn_wp = nullptr, *edge_keys = nullptr;
-  uint32_t* red_block = nullptr;  // [first_ls | first_cpu | first_comm]: the direct first-row tables mode B all-reduces
+  uint32_t *loc_bits = nullptr, *loc_wp = nullptr, *sd_bits[4] = {}, *sd_wp[4] = {}, *fn_bits = nullptr, *fn_wp = nullptr;
+  unsigned long long* edge_keys = nullptr;
+  uint32_t* red_block = nullptr;  // [first_ls | first_cpu | first_comm | v1: first_kind]: the direct first-row tables mode B all-reduces
   size_t red_count = 0;
   std::vector<uint32_t*> col_first, col_rank, col_bits, col_wp;
   int j_loc = 0, j_type = 0, j_file = 0, j_lab0 = 0;
@@ -190,6 +191,7 @@ struct pa_agg {
   uint64_t store_epoch = 0;                  // LRU clock: one tick per ingested batch and per stacktrace request
   uint32_t* h_select = nullptr;              // pinned: 256-bin histogram of a select pass, then a StoreCtl read-back
   uint64_t store_compactions = 0, store_evictions = 0;
+  uint64_t store_frames_sent = 0;            // v1 merge groups: frame ids this member sent in the last store exchange
   uint32_t cid_unknown = 0, cid_missing = 0;  // "unknown" (libpf.UnknownFrame.String()) and "missing stacktrace" (:1561, :1568)
 
   // ---- ring (pinned host), double buffered
@@ -777,7 +779,7 @@ static int upload_descriptors(pa_agg* a, const void* jobs, size_t jb, const void
 
 // v1: the batch's accesses to the `stacks` LRU (parca_reporter.go:224-227): every unique stack of the batch is looked up and, if
 // unknown, added; known ones (evicted ones included) get the batch's access time
-static void launch_store_insert(pa_agg* a, uint32_t min_last_p1) {
+static StoreInsertArgs store_insert_args(pa_agg* a, uint32_t min_last_p1) {
   StoreInsertArgs sa{};
   Counters* ctr = a->d_ctr.as<Counters>();
   sa.ctr = ctr; sa.uniq_row = a->d_uniq_row.as<uint32_t>(); sa.slot_of_row = a->d_slot.as<uint32_t>(); sa.tab = a->d_table.as<StackSlot>();
@@ -789,8 +791,9 @@ static void launch_store_insert(pa_agg* a, uint32_t min_last_p1) {
   sa.cap_frames = a->store_frames; sa.cap_entries = (uint32_t)(a->store_slots - a->store_slots / 4); sa.ctl = a->d_store_ctl.as<StoreCtl>(); sa.ctr_w = ctr;
   sa.stamp = a->d_store_stamp.as<unsigned long long>(); sa.last_row = a->d_v1_last.as<uint32_t>();
   sa.epoch_hi = a->store_epoch << 32; sa.min_last_p1 = min_last_p1;
-  k_store_insert<<<a->G, kThreads, 0, a->s_comp>>>(sa);
+  return sa;
 }
+static void launch_store_insert(pa_agg* a, uint32_t min_last_p1) { k_store_insert<false><<<a->G, kThreads, 0, a->s_comp>>>(store_insert_args(a, min_last_p1)); }
 // the k-th largest of the non-zero keys (k >= 1, at least k of them exist): eight histogram passes from the top byte down
 static int select_kth_largest(pa_agg* a, const unsigned long long* keys, uint64_t n, uint64_t k, unsigned long long* out) {
   cudaStream_t s = a->s_comp;
@@ -966,12 +969,13 @@ static int pass_plan(pa_agg* a, const MergeDims* md) {
   want(&P.first_ls, std::max<size_t>(P.n_labelsets, 1) * 4, 0);
   if (has_cpu) want(&first_cpu, 65536 * 4, 0);
   if (has_comm) want(&first_comm, S * 4, 0);
+  if (v1) want(&a->v1_first_kind, 8 * 4, 0);  // (a merged batch takes the minimum over the shards: the kind columns' dictionary order)
   size_t red_bytes = 0;
   for (auto& r : reqs) red_bytes += r.bytes;
   if (v1) {
     want(&a->v1_ord, Nn * 4); want(&a->v1_ts_vals, Nn * 8); want(&a->v1_id_off, (Nn + 1) * 4);
     a->v1_ids = a->d_v1_ids.as<uint8_t>();  // outlives the arena: pa_agg_last_stack_ids / pa_agg_stacktraces run after the flush
-    want(&a->v1_first_kind, 8 * 4, 0); want(&a->v1_kindrank, 64 * 4); want(&a->v1_kind_order, 64 * 4); want(&a->v1_n_kind_dict, 8 * 4);
+    want(&a->v1_kindrank, 64 * 4); want(&a->v1_kind_order, 64 * 4); want(&a->v1_n_kind_dict, 8 * 4);
   }
   want(&P.rowbits, (NTn / 32 + 2) * 4, 1); want(&P.row_wprefix, (NTn / 32 + 2) * 4);
   if (!md) { want(&P.uniq_slot, Nn * 4); want(&P.uniq_size, Nn * 4); }  // merged: sized by the merged dictionary (merge_impl.hpp)
@@ -988,7 +992,7 @@ static int pass_plan(pa_agg* a, const MergeDims* md) {
   want(&P.fn_bits, (Pn / 32 + 2) * 4); want(&P.fn_wp, (Pn / 32 + 2) * 4);
   want(&a->lo.address, Pn * 8); want(&a->lo.line_off, Pn * 4); want(&a->lo.line_size, Pn * 4); want(&a->lo.line_valid, (Pn / 32 + 2) * 4);
   want(&a->lo.line_no, Pn * 8);
-  if (md) want(&P.edge_keys, (size_t)ncols * 16, 1);
+  if (md) want(&P.edge_keys, (size_t)ncols * 32, 1);
   P.tiles = ReeTiles{};
   P.tiles.n_tiles = (uint32_t)((N + kTileRows - 1) / kTileRows);
   if (!md) { want(&P.tiles.desc, (size_t)ncols * std::max<uint32_t>(P.tiles.n_tiles, 1) * 8, 1); want(&P.tiles.next, (size_t)ncols * 4, 1); }
@@ -1513,7 +1517,7 @@ static int d2h_vec(pa_agg* a, std::vector<uint32_t>& dst, const uint32_t* src, s
 // Buffers of a merged batch (mode B) that are spread over the shards: every shard holds the part that belongs to its rows /
 // its runs / its range of the location-index stream. The plan only needs their total length; merge_impl.hpp copies each
 // shard's part to (placement + part offset).
-enum SliceKind : uint32_t { SL_TS = 1, SL_VALUE, SL_UUID, SL_STOFF, SL_STSIZE, SL_STREAM, SL_RUN_ENDS, SL_RUN_KEYS, SL_VALID };
+enum SliceKind : uint32_t { SL_TS = 1, SL_VALUE, SL_UUID, SL_STOFF, SL_STSIZE, SL_STREAM, SL_RUN_ENDS, SL_RUN_KEYS, SL_VALID, SL_TS_RUNS /* v1: int64 run values */ };
 static BufRef sliced(uint32_t kind, uint32_t col, uint64_t len) { return BufRef{BufRef::SLICED, (const void*)(uintptr_t)(((uint64_t)kind << 16) | col), len}; }
 struct MergeView {
   uint64_t NT;                                            // rows of the merged batch
@@ -1587,7 +1591,6 @@ static int collect_nodes(pa_agg* a, const MergeView* mv, std::vector<Node>& cols
     return rc;
   for (uint32_t i = 0; i < nlab; i++)
     if (c.last_nonnull_plus1[i] && (rc = d2h_vec(a, ord_lab[i], a->cols[i].order, c.n_dict[i]))) return rc;
-  if (mv && v1) return a->fail(PA_EINVAL, "a merged batch needs PA_SCHEMA_V2 shards");
   for (uint32_t t = v1 ? 6 : 0; t < 8; t++) {  // v1: the six string columns stay on the device as dictionary indices
     if (mv) { kind_keys[t] = (*mv->kind_keys)[t]; continue; }
     if ((rc = d2h_vec(a, kind_keys[t], a->cols[nlab + t].run_keys, c.n_runs[nlab + t]))) return rc;
@@ -1704,9 +1707,10 @@ static int collect_nodes(pa_agg* a, const MergeView* mv, std::vector<Node>& cols
   std::sort(labels.begin(), labels.end(), [](const LabelOut& x, const LabelOut& y) { return x.name < y.name; });
   tp2 = now_ms();
 
-  auto ree_run_ends_of = [&](uint32_t col) { return BufRef::dev(a->cols[col].run_ends, (uint64_t)c.n_runs[col] * 4); };
+  auto ree_run_ends_of = [&](uint32_t col) { return runbuf(SL_RUN_ENDS, col, a->cols[col].run_ends, c.n_runs[col], 4); };
   if (v1) {
     // ---- v1 sample record (reporter/arrow.go:274-316, ArrowSamplesField :484-503): label columns first, then the 11 fixed columns
+    // (merged batch: the stacktrace_id dictionary is replicated on every shard, the run-end columns are sliced like the labels)
     for (auto& l : labels) cols.push_back(std::move(l.node));
     const uint32_t c_ord = nlab + 8, c_ts = nlab + 9, nu = c.n_unique;
     {
@@ -1714,7 +1718,7 @@ static int collect_nodes(pa_agg* a, const MergeView* mv, std::vector<Node>& cols
       ids.bufs = {BufRef::dev(a->v1_id_off, ((uint64_t)nu + 1) * 4), BufRef::dev(a->v1_ids, (uint64_t)nu * 16)};
       uint32_t nr = c.n_runs[c_ord];  // run key == stack ordinal == dictionary index
       cols.push_back(ree_node("stacktrace_id", false, (int64_t)N, nr, ree_run_ends_of(c_ord),
-                              dict_node("values", true, nr, 0, BufRef::none(), BufRef::dev(a->cols[c_ord].run_keys, (uint64_t)nr * 4), std::move(ids))));
+                              dict_node("values", true, nr, 0, BufRef::none(), runbuf(SL_RUN_KEYS, c_ord, a->cols[c_ord].run_keys, nr, 4), std::move(ids))));
     }
     cols.push_back(int_node("value", 64, true, false, (int64_t)N, rowbuf(SL_VALUE, a->d_value.p, 8)));
     static const char* names[6] = {"producer", "sample_type", "sample_unit", "period_type", "period_unit", "temporality"};
@@ -1728,8 +1732,8 @@ static int collect_nodes(pa_agg* a, const MergeView* mv, std::vector<Node>& cols
       uint32_t nr = c.n_runs[nlab + t];
       int64_t nulls = t == 5 ? (int64_t)c.n_null[nlab + t] : 0;  // memory samples carry a null temporality
       cols.push_back(ree_node(names[t], false, (int64_t)N, nr, ree_run_ends_of(nlab + t),
-                              dict_node("values", true, nr, nulls, nulls ? BufRef::dev(cp.validity, (nr + 7) / 8) : BufRef::none(),
-                                        BufRef::dev(cp.run_keys, (uint64_t)nr * 4), utf8_node(a, "values", true, strs, nullptr, Ty::Binary))));
+                              dict_node("values", true, nr, nulls, nulls ? validbuf(nlab + t, cp.validity, nr) : BufRef::none(),
+                                        runbuf(SL_RUN_KEYS, nlab + t, cp.run_keys, nr, 4), utf8_node(a, "values", true, strs, nullptr, Ty::Binary))));
     }
     {
       std::vector<int64_t> pv; for (uint32_t k : kind_keys[6]) pv.push_back(a->period_vals[k]);
@@ -1739,7 +1743,7 @@ static int collect_nodes(pa_agg* a, const MergeView* mv, std::vector<Node>& cols
     }
     {
       uint32_t nr = c.n_runs[c_ts];
-      cols.push_back(ree_node("timestamp", false, (int64_t)N, nr, ree_run_ends_of(c_ts), int_node("values", 64, true, true, nr, BufRef::dev(a->v1_ts_vals, (uint64_t)nr * 8))));
+      cols.push_back(ree_node("timestamp", false, (int64_t)N, nr, ree_run_ends_of(c_ts), int_node("values", 64, true, true, nr, runbuf(SL_TS_RUNS, c_ts, a->v1_ts_vals, nr, 8))));
     }
   } else {
   {
@@ -2623,6 +2627,13 @@ int pa_agg_last_kernel_ms(const pa_agg* a, const char* name, double* ms, uint32_
   if (!strcmp(name, "store_compactions") || !strcmp(name, "store_evictions")) {
     if (ms) *ms = 0;
     if (launches) *launches = (uint32_t)(name[6] == 'c' ? a->store_compactions : a->store_evictions);
+    return PA_OK;
+  }
+  // PA_SCHEMA_V1 merge groups (ms is 0): frame ids (4 bytes each) this member sent to the other copies of the store in the last
+  // store exchange of pa_merge_process
+  if (!strcmp(name, "store_frames")) {
+    if (ms) *ms = 0;
+    if (launches) *launches = (uint32_t)std::min<uint64_t>(a->store_frames_sent, 0xFFFFFFFFu);
     return PA_OK;
   }
   return PA_EINVAL;

@@ -1898,12 +1898,13 @@ struct ReeArgs {
   uint32_t kind_dict_mask;   // bit t: kind column t is dictionary encoded
   // mode B (one merged batch over several shards): this shard's rows are the global rows row_base .. row_base+n_rows-1
   uint32_t row_base;         // added to every run end
-  uint32_t* edge_keys;       // [ncols][4] = first key, first null, last key, last null of this shard (count pass); nullptr = off
+  unsigned long long* edge_keys;  // [ncols][4] = first key, first null, last key, last null of this shard (count pass); nullptr = off
   const struct MergeCol* mc; // per column: how many local runs stay in this shard's part + validity bit shift (emit pass); nullptr = off
 };
 struct EdgeCol {   // what one shard contributes to the cross-shard run merge of one REE column
   uint32_t n_runs, n_null, lastnn, n_rows;
-  uint32_t first_key, first_null, last_key, last_null;
+  unsigned long long first_key, last_key;  // 64 bits: the v1 timestamp column's keys are int64
+  uint32_t first_null, last_null;
 };
 struct MergeCol {
   uint32_t keep;       // local runs that stay in this shard's part: n_runs, or n_runs-1 when its last run continues in the next shard
@@ -1954,8 +1955,8 @@ __device__ __forceinline__ void ree_single(const ReeArgs& a, uint32_t c, bool ha
       in[u] = r < end; key[u] = 0; null[u] = true;
       if (in[u]) kf.get(r, key[u], null[u]);
       if (!EMIT && MERGED && in[u]) {
-        if (r == 0) { a.edge_keys[c * 4 + 0] = (uint32_t)key[u]; a.edge_keys[c * 4 + 1] = null[u] ? 1u : 0u; }
-        if (r + 1 == a.n_rows) { a.edge_keys[c * 4 + 2] = (uint32_t)key[u]; a.edge_keys[c * 4 + 3] = null[u] ? 1u : 0u; }
+        if (r == 0) { a.edge_keys[c * 4 + 0] = (unsigned long long)key[u]; a.edge_keys[c * 4 + 1] = null[u] ? 1u : 0u; }
+        if (r + 1 == a.n_rows) { a.edge_keys[c * 4 + 2] = (unsigned long long)key[u]; a.edge_keys[c * 4 + 3] = null[u] ? 1u : 0u; }
       }
     }
 #pragma unroll
@@ -2320,6 +2321,12 @@ struct StoreInsertArgs {
   const uint32_t* last_row;          // [batch table slots] last row of every stack of the batch
   unsigned long long epoch_hi;       // epoch << 32
   uint32_t min_last_p1;              // only stacks with last_row + 1 >= this are stored (a batch with more unique stacks than the cache holds)
+  // merged batch (k_store_insert<true>): the merged dictionary instead of this shard's rows, indexed by merged ordinal
+  const StackSlot* gtab;             // merged table: key and depth of the global first occurrence
+  const uint32_t* g_slot;            // [U] merged table slot of every ordinal
+  const uint32_t* g_last_inv;        // [U] 0xFFFFFFFF - global last row
+  const uint32_t* g_frames;          // frames of the stacks the store lacks, gathered from the shards that hold their first occurrence
+  const unsigned long long* g_foff;  // [U + 1] where each ordinal's frames start in g_frames (an ordinal without frames there: equal neighbours)
 };
 // last occurrence of every stack of the batch (the LRU's access time of its entry)
 __global__ void __launch_bounds__(kThreads) k_last_rows(uint32_t n_rows, const uint32_t* slot_of_row, uint32_t* last_row) {
@@ -2360,7 +2367,9 @@ __global__ void __launch_bounds__(kThreads) k_store_kill(unsigned long long* sta
   for (int o = 16; o > 0; o >>= 1) killed += __shfl_xor_sync(0xFFFFFFFFu, killed, o);
   if ((threadIdx.x & 31) == 0 && killed) atomicSub(&ctl->live, killed);
 }
-// one warp per unique stack of the batch (unique within the launch, so a key is claimed by at most one warp)
+// one warp per unique stack of the batch (unique within the launch, so a key is claimed by at most one warp).
+// MERGED: one replica of a merge group's store; u is the merged ordinal, frames come from the gathered buffer.
+template <bool MERGED>
 __global__ void __launch_bounds__(kThreads) k_store_insert(StoreInsertArgs a) {
   const unsigned full = 0xFFFFFFFFu;
   uint32_t nu = a.ctr->n_unique;
@@ -2368,14 +2377,20 @@ __global__ void __launch_bounds__(kThreads) k_store_insert(StoreInsertArgs a) {
   uint32_t warp = (blockIdx.x * kThreads + threadIdx.x) >> 5, nwarps = (gridDim.x * kThreads) >> 5;
   const Key128 zero{0ull, 0ull};
   for (uint32_t u = warp; u < nu; u += nwarps) {
-    uint32_t r = a.uniq_row[u];
-    uint32_t size = a.nframes[r];
+    uint32_t r = 0, size, lr;
+    if constexpr (MERGED) {
+      size = a.gtab[a.g_slot[u]].size;
+      lr = 0xFFFFFFFFu - a.g_last_inv[u];
+    } else {
+      r = a.uniq_row[u];
+      size = a.nframes[r];
+      lr = a.last_row[a.slot_of_row[r]];
+    }
     unsigned long long off = 0;
     int fresh = 0;
-    const uint32_t lr = a.last_row[a.slot_of_row[r]];
     if (lr + 1u < a.min_last_p1) continue;  // warp-uniform: older than everything the cache will hold after this batch
     if (lane == 0) {
-      Key128 k = a.tab[a.slot_of_row[r]].key;
+      Key128 k = MERGED ? a.gtab[a.g_slot[u]].key : a.tab[a.slot_of_row[r]].key;
       uint32_t idx = kNull;
       if (key_zero(k)) {
         idx = a.mask + 1;
@@ -2417,11 +2432,20 @@ __global__ void __launch_bounds__(kThreads) k_store_insert(StoreInsertArgs a) {
     fresh = __shfl_sync(full, fresh, 0);
     if (!fresh) continue;
     off = __shfl_sync(full, off, 0);
-    const unsigned long long base = a.frame_off[r];
-    for (uint32_t j = lane; j < size; j += 32) {
-      unsigned long long fid = frame_at(a.frames, base + j, a.narrow);
-      if (fid >= a.n_frames_registered) { atomicOr(&a.ctr_w->err, ERR_BAD_FRAME_ID); fid = 0; }
-      a.arena[off + j] = (uint32_t)fid;
+    if constexpr (MERGED) {  // the frames were checked where they were packed (k_store_pack)
+      const unsigned long long base = a.g_foff[u];
+      if (a.g_foff[u + 1] - base != size) {  // not in the gathered set: a logic error, reported instead of storing garbage
+        if (lane == 0) atomicOr(&a.ctr_w->err, ERR_MERGE_LOOKUP);
+        continue;
+      }
+      for (uint32_t j = lane; j < size; j += 32) a.arena[off + j] = a.g_frames[base + j];
+    } else {
+      const unsigned long long base = a.frame_off[r];
+      for (uint32_t j = lane; j < size; j += 32) {
+        unsigned long long fid = frame_at(a.frames, base + j, a.narrow);
+        if (fid >= a.n_frames_registered) { atomicOr(&a.ctr_w->err, ERR_BAD_FRAME_ID); fid = 0; }
+        a.arena[off + j] = (uint32_t)fid;
+      }
     }
   }
 }
@@ -2862,10 +2886,11 @@ __global__ void __launch_bounds__(kThreads) k_min_u32(uint32_t* dst, const uint3
 // non-empty shard when both border rows are non-null and carry the same key (BinaryDictionaryRunEndBuilder.Append,
 // reporter/arrow.go:97-131: a row extends the current run iff the previous value is non-null and byte-equal). The
 // continued run is written by the shard where it ENDS; the shard where it starts drops its last run.
-__global__ void __launch_bounds__(kThreads) k_edges_pack(const Counters* ctr, const uint32_t* edge_keys, uint32_t ncols, uint32_t row_base, uint32_t n_rows, EdgeCol* out) {
+__global__ void __launch_bounds__(kThreads) k_edges_pack(const Counters* ctr, const unsigned long long* edge_keys, uint32_t ncols, uint32_t row_base, uint32_t n_rows, EdgeCol* out) {
   for (uint32_t c = threadIdx.x; c < ncols; c += blockDim.x) {
     const uint32_t lnn = ctr->last_nonnull_plus1[c];
-    out[c] = EdgeCol{ctr->n_runs[c], ctr->n_null[c], lnn ? row_base + lnn : 0u, n_rows, edge_keys[c * 4 + 0], edge_keys[c * 4 + 1], edge_keys[c * 4 + 2], edge_keys[c * 4 + 3]};
+    out[c] = EdgeCol{ctr->n_runs[c], ctr->n_null[c], lnn ? row_base + lnn : 0u, n_rows, edge_keys[c * 4 + 0], edge_keys[c * 4 + 2],
+                     (uint32_t)edge_keys[c * 4 + 1], (uint32_t)edge_keys[c * 4 + 3]};
   }
 }
 __global__ void __launch_bounds__(kThreads) k_merge_cols(const EdgeCol* edges /*[world][ncols]*/, uint32_t world, uint32_t me, uint32_t ncols,
@@ -2890,6 +2915,87 @@ __global__ void __launch_bounds__(kThreads) k_merge_cols(const EdgeCol* edges /*
     }
     // the counters now describe the MERGED column (identical on every shard)
     ctr_w->n_runs[c] = base; ctr_w->n_null[c] = nulls; ctr_w->last_nonnull_plus1[c] = lastnn;
+  }
+}
+
+// ---- v1 merged batch: the stacktrace_id dictionary and the known-stacks store, both replicated on every shard. Every shard
+// applies the same merged accesses to its copy of the store, so the copies stay identical; only the frames of the stacks the
+// store lacks cross between the shards, each sent by the shard that holds the stack's global first occurrence.
+// dictionary values of the stacktrace_id column: the merged ids in ordinal order, as the hash kernels write them per row
+__global__ void __launch_bounds__(kThreads) k_merged_ids(const Counters* ctr, const StackSlot* gtab, const uint32_t* g_slot, uint8_t* out, int* offsets) {
+  const uint32_t nu = ctr->n_unique;
+  for (uint32_t u = blockIdx.x * kThreads + threadIdx.x; u <= nu; u += gridDim.x * kThreads) {
+    offsets[u] = (int)(16u * u);
+    if (u < nu) { const Key128 k = gtab[g_slot[u]].key; *reinterpret_cast<ulonglong2*>(out + 16ull * u) = make_ulonglong2(bswap64(k.hi), bswap64(k.lo)); }
+  }
+}
+// last global row of every merged stack this shard holds, inverted: one all-reduce(min) over the shards gives the global last row
+__global__ void __launch_bounds__(kThreads) k_merged_last_rows(uint32_t n_rows, const uint32_t* slot_of_row, const StackSlot* ltab, uint32_t row_base, uint32_t* last_inv) {
+  for (uint32_t i = blockIdx.x * kThreads + threadIdx.x; i < n_rows; i += gridDim.x * kThreads) {  // from the last row down, as k_last_rows
+    const uint32_t r = n_rows - 1u - i, s = slot_of_row[r];
+    if (s == kNull) continue;
+    const uint32_t o = ltab[s].ordinal, v = 0xFFFFFFFFu - (row_base + r);
+    if (last_inv[o] > v) atomicMin(&last_inv[o], v);
+  }
+}
+// select keys of the U >= capacity case (k_batch_stamps over merged ordinals)
+__global__ void __launch_bounds__(kThreads) k_merged_stamps(const Counters* ctr, const uint32_t* last_inv, unsigned long long* out) {
+  const uint32_t nu = ctr->n_unique;
+  for (uint32_t u = blockIdx.x * kThreads + threadIdx.x; u < nu; u += gridDim.x * kThreads) out[u] = (unsigned long long)(0xFFFFFFFFu - last_inv[u]) + 1ull;
+}
+// frames (depth) each merged stack contributes to the exchange: those the insert may write — stacks it stores (last row + 1 >=
+// min_last_p1) that the store does not hold live (after a clear: all of them). Every replica computes the same.
+__global__ void __launch_bounds__(kThreads) k_store_need(const Counters* ctr, const StackSlot* gtab, const uint32_t* g_slot, const uint32_t* last_inv,
+                                                         uint32_t min_last_p1, const StoreSlot* st, uint32_t mask, const unsigned long long* stamp,
+                                                         uint32_t* need) {
+  const uint32_t nu = ctr->n_unique;
+  for (uint32_t u = blockIdx.x * kThreads + threadIdx.x; u < nu; u += gridDim.x * kThreads) {
+    const StackSlot e = gtab[g_slot[u]];
+    bool n = (0xFFFFFFFFu - last_inv[u]) + 1u >= min_last_p1;
+    if (n) {
+      const uint32_t sl = store_find(st, mask, e.key);
+      n = sl == kNull || st[sl].size == kNull || stamp[sl] == 0;
+    }
+    need[u] = n ? e.size : 0u;
+  }
+}
+struct StoreFramesF {  // where each merged stack's frames start in the gathered buffer: exclusive scan of k_store_need
+  typedef unsigned long long T;
+  const Counters* ctr;
+  const uint32_t* need;
+  unsigned long long* foff;
+  __device__ uint32_t n() const { return ctr->n_unique; }
+  __device__ unsigned long long value(uint32_t u) const { return need[u]; }
+  __device__ void emit(uint32_t u, unsigned long long ex, unsigned long long) const { foff[u] = ex; }
+  __device__ void total(int, unsigned long long t) const { foff[ctr->n_unique] = t; }
+};
+// every rank's share of the gathered buffer: rank r sends the stacks whose global first row lies in its rows (a contiguous
+// range of ordinals, see k_won_range), so its block starts at foff[first ordinal at or after row_base[r]]
+struct RankRows { uint32_t base[kMaxWorld + 1]; };
+__global__ void k_rank_bounds(const Counters* ctr, const uint32_t* g_row, const unsigned long long* foff, RankRows rr, uint32_t world, unsigned long long* out) {
+  const uint32_t r = threadIdx.x, nu = ctr->n_unique;
+  if (r > world) return;
+  uint32_t lo = 0, hi = nu;
+  while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (g_row[mid] < rr.base[r]) lo = mid + 1; else hi = mid; }
+  out[r] = foff[lo];
+}
+// this shard's block: the frames of its won stacks that k_store_need selected, from their (local) first occurrence
+__global__ void __launch_bounds__(kThreads) k_store_pack(const MergeCtl* mc, const uint32_t* g_row, uint32_t row_base, const uint32_t* need,
+                                                         const unsigned long long* foff, const unsigned long long* frames, const unsigned long long* frame_off,
+                                                         uint32_t n_frames_registered, uint32_t narrow, uint32_t* out, Counters* ctr_w) {
+  const uint32_t o0 = mc->ord0, o1 = mc->ord1;
+  const unsigned long long base0 = foff[o0];
+  const int lane = threadIdx.x & 31;
+  const uint32_t warp = (blockIdx.x * kThreads + threadIdx.x) >> 5, nwarps = (gridDim.x * kThreads) >> 5;
+  for (uint32_t u = o0 + warp; u < o1; u += nwarps) {
+    const uint32_t size = need[u];
+    if (!size) continue;
+    const unsigned long long src = frame_off[g_row[u] - row_base], dst = foff[u] - base0;
+    for (uint32_t j = lane; j < size; j += 32) {
+      unsigned long long fid = frame_at(frames, src + j, narrow);
+      if (fid >= n_frames_registered) { atomicOr(&ctr_w->err, ERR_BAD_FRAME_ID); fid = 0; }
+      out[dst + j] = (uint32_t)fid;
+    }
   }
 }
 

@@ -9,7 +9,9 @@
 //   all-to-all   (id128, global first row, depth) of each shard's unique stacks to the id's owner     U_local x 24 B
 //   all-gather   the owners' deduplicated lists (every shard then ranks them identically)             U x 24 B
 //   all-reduce   min over the frame-indexed first-position table and the direct label tables          (P + L + 64k + S) x 4 B
-//   all-gather   thread-id lists, per-column run edges (count, first / last key)                      T x 8 B + cols x 32 B
+//   all-gather   thread-id lists, per-column run edges (count, first / last key)                      T x 8 B + cols x 40 B
+//   v1 groups (replicated known-stacks store): all-reduce(min) of each merged stack's inverted last row  U x 4 B
+//                and all-gather-v of the frames of the stacks the store lacks                          4 B per frame (0 in steady state)
 // Invariants reproduced: first-occurrence order of every dictionary (arrow_v2.go:191, :302; parca_reporter.go:425),
 // run merging across shard borders (arrow.go:97-131).
 //
@@ -75,9 +77,12 @@ struct MergeBufs {
   DBuf ctl;        // MergeCtl + owner-table control words + merged-table control words + per-owner counters / cursors
   DBuf send, recv, otab, oclaimed, ouniq, glist, gtab, gclaimed, g_uniq_row, g_uniq_slot, g_uniq_size;
   DBuf tid_list, tid_all, edges, edges_all, mcols, mcols_all, gather_scratch, kind_all, vwords, vwords_all;
+  // v1 groups only: stacktrace_id offsets, and the replicated store's update (last rows, frames exchange) and requests
+  DBuf v1_off, v1_last, v1_need, v1_foff, v1_bounds, v1_send, v1_frames, v1_ids_req;
   void release() {
     DBuf* all[] = {&ctl, &send, &recv, &otab, &oclaimed, &ouniq, &glist, &gtab, &gclaimed, &g_uniq_row, &g_uniq_slot, &g_uniq_size,
-                   &tid_list, &tid_all, &edges, &edges_all, &mcols, &mcols_all, &gather_scratch, &kind_all, &vwords, &vwords_all};
+                   &tid_list, &tid_all, &edges, &edges_all, &mcols, &mcols_all, &gather_scratch, &kind_all, &vwords, &vwords_all,
+                   &v1_off, &v1_last, &v1_need, &v1_foff, &v1_bounds, &v1_send, &v1_frames, &v1_ids_req};
     for (DBuf* b : all) b->release();
   }
 };
@@ -180,6 +185,12 @@ namespace pa {
 static bool lz4_gpu_member(const pa_agg* m) { return m->cfg.ipc_compression == PA_IPC_LZ4_FRAME_GPU; }
 static const char kLz4Mixed[] = "a merge group builds LZ4_FRAME records only when every member uses PA_IPC_LZ4_FRAME_GPU, and plain ones when none does: "
                                 "this group mixes PA_IPC_LZ4_FRAME_GPU members with other members";
+// Every member of a group uses the same schema; v1 members also need the same store size, since each holds a full copy of the
+// group's store (refused like a mixed LZ4 mode).
+static const char kSchemaMixed[] = "a merge group builds one record schema: this group mixes PA_SCHEMA_V1 and PA_SCHEMA_V2 members";
+static const char kStoreMismatch[] = "the members of a PA_SCHEMA_V1 merge group each hold a copy of the group's known-stacks store: "
+                                     "their stack_cache_entries / stack_cache_frames must be equal (left at 0, both follow max_samples: "
+                                     "members with different rings then need explicit, equal sizes)";
 static cudaStream_t mstream(pa_merge* g, size_t i) { return g->members[i]->s_comp; }
 // An in-process group on one device runs every member on ONE stream while a merge call is active, so that every copy between
 // members is stream-ordered (NCCL groups keep one stream per member: the collectives order them).
@@ -707,19 +718,30 @@ static int merge_process_once(pa_merge* g, bool* retry) {
     // every local stack adopts the merged (ordinal, offset, size); rows pick them up; this shard's range of the stream
     const int Gl = small_grid(a, std::min<uint64_t>(std::max<uint64_t>(a->N, 1), P.cap / 2));
     k_local_adopt<<<Gl, kThreads, 0, s>>>(a->d_table.as<StackSlot>(), P.claimed, &ctr->n_claimed, gtab, gmask, ctl + CTL_MERGED, &ctr->err);
-    k_rows_materialize<<<a->G, kThreads, 0, s>>>((uint32_t)a->N, a->d_slot.as<uint32_t>(), a->d_table.as<StackSlot>(), a->d_stoff.as<int>(), a->d_stsize.as<int>(), nullptr);
-    const uint64_t ucap = std::min<uint64_t>(a->d_ustream.cap / 4, 0x7FFFFFFFull);
+    k_rows_materialize<<<a->G, kThreads, 0, s>>>((uint32_t)a->N, a->d_slot.as<uint32_t>(), a->d_table.as<StackSlot>(), a->d_stoff.as<int>(), a->d_stsize.as<int>(),
+                                                 P.v1 ? a->v1_ord : nullptr);
+    // (v1 has no location-index stream: the won range only tells which stacks' frames this shard sends to the store update)
+    const uint64_t ucap = P.v1 ? 0x7FFFFFFFull : std::min<uint64_t>(a->d_ustream.cap / 4, 0x7FFFFFFFull);
     k_won_range<<<1, 32, 0, s>>>(urow, uslot, gtab, ctr, (uint32_t)P.row_base, (uint32_t)a->N, (uint32_t)ucap, (MergeCtl*)(ctl + CTL_MERGE), ctr);
-    k_gather_won<<<a->G, kThreads, 0, s>>>((const MergeCtl*)(ctl + CTL_MERGE), urow, uslot, gtab, (uint32_t)P.row_base, a->src_frames, a->d_foff.as<unsigned long long>(),
-                                           P.n_frames, a->d_ustream.as<uint32_t>(), a->loc_first, ctr, a->idb == 4 ? 1u : 0u);
+    if (P.v1) {  // the stacktrace_id dictionary, replicated: every shard writes the merged ids from the merged table
+      MCK(a->d_v1_ids.ensure(Un * 16));
+      MCK(mb.v1_off.ensure((Un + 1) * 4));
+      a->v1_ids = a->d_v1_ids.as<uint8_t>();
+      a->v1_id_off = mb.v1_off.as<int>();
+      k_merged_ids<<<small_grid(a, Un + 1), kThreads, 0, s>>>(ctr, gtab, uslot, a->v1_ids, a->v1_id_off);
+    } else {
+      k_gather_won<<<a->G, kThreads, 0, s>>>((const MergeCtl*)(ctl + CTL_MERGE), urow, uslot, gtab, (uint32_t)P.row_base, a->src_frames, a->d_foff.as<unsigned long long>(),
+                                             P.n_frames, a->d_ustream.as<uint32_t>(), a->loc_first, ctr, a->idb == 4 ? 1u : 0u);
+    }
     a->tm[T_RANK].launches += 8;
     MCK(cudaEventRecord(a->tm[T_RANK].b, s));
   }
-  // ---- first positions of frames / first rows of label values: one all-reduce(min) each
+  // ---- first positions of frames (v2) / first rows of label values (v1: and of sample kinds): one all-reduce(min) each
+  const bool v1 = g->members[0]->P.v1;
   {
     std::vector<uint32_t*> lf(L), rb(L);
     for (size_t i = 0; i < L; i++) { lf[i] = g->members[i]->loc_first; rb[i] = g->members[i]->P.red_block; }
-    if ((rc = t_allreduce_min(g, lf, g->members[0]->P.Pn))) return rc;
+    if (!v1 && (rc = t_allreduce_min(g, lf, g->members[0]->P.Pn))) return rc;
     if ((rc = t_allreduce_min(g, rb, g->members[0]->P.red_count))) return rc;
   }
   // ---- dictionaries (identical on every shard), run counts, run edges
@@ -731,7 +753,7 @@ static int merge_process_once(pa_merge* g, bool* retry) {
     MCK(cudaSetDevice(a->device));
     cudaStream_t s = a->s_comp;
     MergeBufs& mb = g->mb[i];
-    if ((rc = pass_locations(a))) return g->fail(rc, a->err);
+    if (!v1 && (rc = pass_locations(a))) return g->fail(rc, a->err);  // (the v1 record has no location or function dictionaries)
     if ((rc = pass_labels_count(a, s))) return g->fail(rc, a->err);
     MCK(mb.edges.ensure(std::max<size_t>((size_t)ncols * sizeof(EdgeCol), 256)));
     MCK(mb.edges_all.ensure(std::max<size_t>((size_t)W * ncols * sizeof(EdgeCol), 256)));
@@ -778,6 +800,163 @@ static int merge_process_once(pa_merge* g, bool* retry) {
   return PA_OK;
 }
 
+// ---- v1 groups: every member holds a full copy of the group's known-stacks store ---------------------------------------
+// A group of v1 members behaves like ONE v1 aggregator fed [shard 0's rows, shard 1's rows, ...]: each member applies the
+// merged batch's accesses to its copy (v1_store_update's steps, over merged ordinals), so the copies stay identical and each
+// one stays a valid store of its own member. Exchanged per interval: the global last row of every merged stack (all-reduce(min)
+// over U words), and the frames of the stacks the store lacks, each sent by the shard that holds its global first occurrence
+// (all-gather-v; near zero in steady state). Every decision below depends only on replicated state, so every rank takes it.
+
+// the frames the insert may need (k_store_need on the store as it is now), gathered into every member's v1_frames
+static int store_frames_exchange(pa_merge* g, uint32_t min_last_p1) {
+  const size_t L = g->members.size();
+  const uint32_t W = g->world;
+  const uint64_t U = g->members[0]->h_ctr.n_unique;
+  std::vector<std::vector<uint64_t>> bounds(L, std::vector<uint64_t>(W + 1));
+  RankRows rr{};
+  for (uint32_t r = 0; r <= W; r++) rr.base[r] = (uint32_t)g->row_base[r];
+  for (size_t i = 0; i < L; i++) {
+    pa_agg* a = g->members[i];
+    MCK(cudaSetDevice(a->device));
+    cudaStream_t s = a->s_comp;
+    MergeBufs& mb = g->mb[i];
+    Counters* ctr = a->d_ctr.as<Counters>();
+    MCK(mb.v1_need.ensure(std::max<uint64_t>(U, 1) * 4));
+    MCK(mb.v1_foff.ensure((U + 1) * 8));
+    MCK(mb.v1_bounds.ensure((W + 1) * 8));
+    k_store_need<<<small_grid(a, U), kThreads, 0, s>>>(ctr, mb.gtab.as<StackSlot>(), mb.g_uniq_slot.as<uint32_t>(), mb.v1_last.as<uint32_t>(), min_last_p1,
+                                                       a->d_store.as<StoreSlot>(), (uint32_t)(a->store_slots - 1), a->d_store_stamp.as<unsigned long long>(),
+                                                       mb.v1_need.as<uint32_t>());
+    launch_scan(a, StoreFramesF{ctr, mb.v1_need.as<uint32_t>(), mb.v1_foff.as<unsigned long long>()}, 1, a->tm[T_RANK], small_grid(a, U), s, a->d_partial);
+    k_rank_bounds<<<1, kMaxWorld + 32, 0, s>>>(ctr, mb.g_uniq_row.as<uint32_t>(), mb.v1_foff.as<unsigned long long>(), rr, W, mb.v1_bounds.as<unsigned long long>());
+    MCK(cudaMemcpyAsync(bounds[i].data(), mb.v1_bounds.p, (W + 1) * 8, cudaMemcpyDeviceToHost, s));
+  }
+  int rc = msync(g);
+  if (rc) return rc;
+  const std::vector<uint64_t>& b = bounds[0];  // identical on every member
+  std::vector<uint64_t> count(W), displ(W);
+  for (uint32_t r = 0; r < W; r++) { displ[r] = b[r] * 4; count[r] = (b[r + 1] - b[r]) * 4; }
+  std::vector<const void*> src(L);
+  std::vector<void*> dst(L);
+  for (size_t i = 0; i < L; i++) {
+    pa_agg* a = g->members[i];
+    MCK(cudaSetDevice(a->device));
+    MergeBufs& mb = g->mb[i];
+    const uint32_t me = g->ranks[i];
+    MCK(mb.v1_send.ensure(std::max<uint64_t>(count[me], 256)));
+    MCK(mb.v1_frames.ensure(std::max<uint64_t>(b[W] * 4, 256)));
+    k_store_pack<<<a->G, kThreads, 0, a->s_comp>>>((const MergeCtl*)(mb.ctl.as<uint32_t>() + CTL_MERGE), mb.g_uniq_row.as<uint32_t>(), (uint32_t)g->row_base[me],
+                                                   mb.v1_need.as<uint32_t>(), mb.v1_foff.as<unsigned long long>(), a->src_frames, a->d_foff.as<unsigned long long>(),
+                                                   a->P.n_frames, a->idb == 4 ? 1u : 0u, mb.v1_send.as<uint32_t>(), a->d_ctr.as<Counters>());
+    a->store_frames_sent += count[me] / 4;
+    src[i] = mb.v1_send.p; dst[i] = mb.v1_frames.p;
+  }
+  return b[W] ? t_allgatherv(g, src, dst, count, displ) : PA_OK;
+}
+
+// v1_store_update for every member's copy, after the merged pass (h_ctr holds the merged counters)
+static int merge_store_update(pa_merge* g) {
+  const size_t L = g->members.size();
+  const uint64_t U = g->members[0]->h_ctr.n_unique, C = g->members[0]->store_entries;
+  int rc;
+  // ---- global last row of every merged stack
+  std::vector<uint32_t*> last(L);
+  for (size_t i = 0; i < L; i++) {
+    pa_agg* a = g->members[i];
+    MCK(cudaSetDevice(a->device));
+    MergeBufs& mb = g->mb[i];
+    if (++a->store_epoch >= (1ull << 32)) return g->fail(a->fail(PA_ERANGE, "stack store: access clock overflow"), a->err);
+    a->store_frames_sent = 0;
+    MCK(mb.v1_last.ensure(std::max<uint64_t>(U, 1) * 4));
+    MCK(cudaMemsetAsync(mb.v1_last.p, 0xFF, U * 4, a->s_comp));
+    k_merged_last_rows<<<a->G, kThreads, 0, a->s_comp>>>((uint32_t)a->N, a->d_slot.as<uint32_t>(), a->d_table.as<StackSlot>(), (uint32_t)a->P.row_base, mb.v1_last.as<uint32_t>());
+    last[i] = mb.v1_last.as<uint32_t>();
+  }
+  if ((rc = t_allreduce_min(g, last, U))) return rc;
+  // ---- room: the U >= C batch keeps its C stacks seen last (the store starts over), otherwise compaction when needed
+  uint32_t min_last_p1 = 0;
+  bool cleared = U >= C;
+  for (size_t i = 0; i < L; i++) {
+    pa_agg* a = g->members[i];
+    MCK(cudaSetDevice(a->device));
+    if (cleared) {  // select keys in v1_foff: it is (U + 1) x 8 bytes, and the frames exchange below only starts filling it
+      MergeBufs& mb = g->mb[i];
+      MCK(mb.v1_foff.ensure((U + 1) * 8));
+      k_merged_stamps<<<small_grid(a, U), kThreads, 0, a->s_comp>>>(a->d_ctr.as<Counters>(), last[i], mb.v1_foff.as<unsigned long long>());
+      unsigned long long t = 0;
+      if ((rc = select_kth_largest(a, mb.v1_foff.as<unsigned long long>(), U, C, &t)) || (rc = store_clear(a))) return g->fail(rc, a->err);
+      min_last_p1 = (uint32_t)t;
+      a->store_evictions++;
+    } else {
+      StoreCtl ctl{};
+      if ((rc = store_ctl_read(a, &ctl))) return g->fail(rc, a->err);
+      const uint64_t phys = a->store_slots - a->store_slots / 4;
+      if (ctl.entries > ctl.live && (ctl.entries + U > phys || ctl.used_frames + a->h_ctr.n_indices64 > a->store_frames) && (rc = store_compact(a))) return g->fail(rc, a->err);
+    }
+  }
+  if ((rc = store_frames_exchange(g, min_last_p1))) return rc;
+  // ---- insert; out of slots or frame space: compaction, then a clear (which needs every stack's frames again)
+  StoreCtl ctl{};
+  for (int attempt = 0; attempt < 3; attempt++) {
+    bool overflow = false;
+    for (size_t i = 0; i < L; i++) {
+      pa_agg* a = g->members[i];
+      MCK(cudaSetDevice(a->device));
+      MergeBufs& mb = g->mb[i];
+      Counters* ctr = a->d_ctr.as<Counters>();
+      MCK(cudaMemsetAsync(&ctr->store_overflow, 0, 4, a->s_comp));
+      StoreInsertArgs sa = store_insert_args(a, min_last_p1);
+      sa.gtab = mb.gtab.as<StackSlot>(); sa.g_slot = mb.g_uniq_slot.as<uint32_t>(); sa.g_last_inv = last[i];
+      sa.g_frames = mb.v1_frames.as<uint32_t>(); sa.g_foff = mb.v1_foff.as<unsigned long long>();
+      k_store_insert<true><<<a->G, kThreads, 0, a->s_comp>>>(sa);
+      MCK(cudaMemcpyAsync(a->h_ctr_pinned, ctr, sizeof(Counters), cudaMemcpyDeviceToHost, a->s_comp));
+      if ((rc = store_ctl_read(a, &ctl))) return g->fail(rc, a->err);
+      MCK(cudaGetLastError());
+      a->h_ctr.err |= a->h_ctr_pinned->err;
+      overflow |= a->h_ctr_pinned->store_overflow != 0;
+    }
+    if (!overflow || attempt == 2) break;
+    const bool compact = ctl.entries > ctl.live && !cleared && attempt == 0;
+    for (size_t i = 0; i < L; i++) {
+      pa_agg* a = g->members[i];
+      MCK(cudaSetDevice(a->device));
+      if (compact) { if ((rc = store_compact(a))) return g->fail(rc, a->err); }
+      else { if ((rc = store_clear(a))) return g->fail(rc, a->err); a->store_evictions++; }
+    }
+    if (!compact) {
+      cleared = true;
+      if ((rc = store_frames_exchange(g, min_last_p1))) return rc;
+    }
+  }
+  // ---- evict everything but the C entries accessed last
+  if (ctl.live > C) {
+    for (size_t i = 0; i < L; i++) {
+      pa_agg* a = g->members[i];
+      MCK(cudaSetDevice(a->device));
+      unsigned long long t = 0;
+      if ((rc = select_kth_largest(a, a->d_store_stamp.as<unsigned long long>(), a->store_slots + 2, C, &t))) return g->fail(rc, a->err);
+      k_store_kill<<<small_grid(a, a->store_slots + 2), kThreads, 0, a->s_comp>>>(a->d_store_stamp.as<unsigned long long>(), a->store_slots + 2, t, a->d_store_ctl.as<StoreCtl>());
+      MCK(cudaStreamSynchronize(a->s_comp));
+      MCK(cudaGetLastError());
+      a->store_evictions++;
+    }
+  }
+  // ---- every rank must agree on the outcome: a bad frame id is seen only by the shard that packs that stack's frames
+  std::vector<const void*> esrc(L);
+  for (size_t i = 0; i < L; i++) esrc[i] = &g->members[i]->d_ctr.as<Counters>()->err;
+  std::vector<uint8_t> hb;
+  if ((rc = t_allgather_host(g, esrc, 4, hb))) return rc;
+  uint32_t err_any = 0;
+  for (uint32_t r = 0; r < g->world; r++) err_any |= ((const uint32_t*)hb.data())[r];
+  for (size_t i = 0; i < L; i++) {
+    pa_agg* a = g->members[i];
+    a->last_unique = U;
+    a->h_ctr.err |= err_any;
+    if ((rc = check_batch_errors(a, a->h_ctr.err))) return g->fail(rc, a->err);
+  }
+  return PA_OK;
+}
+
 static int merge_process(pa_merge* g) {
   const size_t L = g->members.size();
   const uint32_t W = g->world;
@@ -787,7 +966,6 @@ static int merge_process(pa_merge* g) {
   for (size_t i = 0; i < L; i++) {
     pa_agg* a = g->members[i];
     if (a->staged < 0) return g->fail(PA_EINVAL, "every member needs a staged batch (pa_agg_stage) before pa_merge_process");
-    if (a->cfg.schema != PA_SCHEMA_V2) return g->fail(PA_EINVAL, "a merged batch needs PA_SCHEMA_V2 members");
     MCK(cudaSetDevice(a->device));
     a->processed = false;
     a->merged_part = true;
@@ -796,14 +974,15 @@ static int merge_process(pa_merge* g) {
   StreamShare share(g);
   auto restore = [] {};
   // ---- rows of every shard -> global row ranges; registrations must be identical (ids are global)
-  struct Dims { uint64_t n, nf; uint32_t ncols, nlab, n_frames, n_cstr, n_labelsets, n_funcs, lz4; };
+  struct Dims { uint64_t n, nf, store_entries, store_frames; uint32_t ncols, nlab, n_frames, n_cstr, n_labelsets, n_funcs, lz4, schema; };
   std::vector<const void*> src(L);
   std::vector<uint8_t> hb;
   rc = PA_OK;
   for (size_t i = 0; i < L && !rc; i++) {
     pa_agg* a = g->members[i];
     cudaSetDevice(a->device);
-    Dims d{a->N, a->NF, (uint32_t)a->cols.size(), a->n_label_cols, a->P.n_frames, a->P.n_cstr, a->P.n_labelsets, a->P.n_funcs, g->lz4 ? 1u : 0u};
+    Dims d{a->N, a->NF, a->store_entries, a->store_frames, (uint32_t)a->cols.size(), a->n_label_cols, a->P.n_frames, a->P.n_cstr, a->P.n_labelsets, a->P.n_funcs,
+           g->lz4 ? 1u : 0u, (uint32_t)a->cfg.schema};
     if (g->mb[i].gather_scratch.ensure(std::max<size_t>((size_t)(W + 1) * sizeof(Dims), 256)) != cudaSuccess) { rc = g->fail(PA_ENOMEM, "device allocation failed"); break; }
     // staged through the tail of the gather scratch (the head receives the gathered block)
     uint8_t* mine = g->mb[i].gather_scratch.as<uint8_t>() + (size_t)W * sizeof(Dims);
@@ -813,8 +992,15 @@ static int merge_process(pa_merge* g) {
   if (!rc) rc = t_allgather_host(g, src, sizeof(Dims), hb);
   if (rc) { restore(); return rc; }
   const Dims* dims = (const Dims*)hb.data();
-  for (uint32_t r = 0; r < W; r++)  // one member per process: the group's mode is settled here, before any work
+  for (uint32_t r = 0; r < W; r++) {  // one member per process: the group's modes are settled here, before any work
     if (dims[r].lz4 != dims[0].lz4) { restore(); return g->fail(PA_EINVAL, kLz4Mixed); }
+    if (dims[r].schema != dims[0].schema) { restore(); return g->fail(PA_EINVAL, kSchemaMixed); }
+    if (dims[0].schema == PA_SCHEMA_V1 && (dims[r].store_entries != dims[0].store_entries || dims[r].store_frames != dims[0].store_frames)) {
+      restore();
+      return g->fail(PA_EINVAL, kStoreMismatch);
+    }
+  }
+  const bool v1 = dims[0].schema == PA_SCHEMA_V1;
   g->n_rows.assign(W, 0); g->nf.assign(W, 0); g->row_base.assign(W + 1, 0);
   g->NT = 0; g->NFT = 0;
   for (uint32_t r = 0; r < W; r++) {
@@ -828,8 +1014,12 @@ static int merge_process(pa_merge* g) {
   g->row_base[W] = g->NT;
   g->ncols = dims[0].ncols;
   if (g->NT > 0x7FFFFFFFull) { restore(); return g->fail(PA_ERANGE, "merged batch exceeds the int32 row limit of run ends / ListView offsets"); }
-  if (g->NT == 0) {
-    for (size_t i = 0; i < L; i++) { g->members[i]->processed = true; memset(&g->members[i]->h_ctr, 0, sizeof(Counters)); }
+  if (g->NT == 0) {  // (like one aggregator's empty batch: no access to the store)
+    for (size_t i = 0; i < L; i++) {
+      pa_agg* a = g->members[i];
+      a->processed = true; a->last_unique = 0; a->store_frames_sent = 0;
+      memset(&a->h_ctr, 0, sizeof(Counters));
+    }
     restore();
     g->processed = true;
     return PA_OK;
@@ -844,11 +1034,12 @@ static int merge_process(pa_merge* g) {
   restore();
   if (rc) return rc;
   if (retry) return g->fail(PA_ENOMEM, "stack / thread-id table overflow");
-  g->ms_total = now_ms() - t0;
   for (size_t i = 0; i < L; i++) {
     pa_agg* a = g->members[i];
     if ((rc = check_batch_errors(a, a->h_ctr.err))) return g->fail(rc, a->err);
   }
+  if (v1 && (rc = merge_store_update(g))) return rc;
+  g->ms_total = now_ms() - t0;
   for (size_t i = 0; i < L; i++) { remember_sizes(g->members[i]); g->members[i]->processed = true; }
   g->processed = true;
   return PA_OK;
@@ -896,7 +1087,7 @@ static int merge_plan(pa_merge* g, uint64_t* ipc_len) {
       if (n) MCK(cudaMemcpyAsync(mine + off, a->cols[nlab + t].run_keys, n, cudaMemcpyDeviceToDevice, a->s_comp));
       off += n;
     }
-    for (uint32_t c = 0; c < nlab; c++) {
+    for (uint32_t c = 0; c < ncols; c++) {  // the label columns, and v1's temporality
       const MergeCol mc = g->cols_all[(size_t)me * ncols + c];
       if (!a->cols[c].validity || !mc.keep) continue;
       const uint32_t last = (mc.vshift + mc.keep - 1) >> 5;
@@ -925,7 +1116,7 @@ static int merge_plan(pa_merge* g, uint64_t* ipc_len) {
   MCK(cudaSetDevice(a0->device));
   MergeView mv{g->NT, &g->kind_keys};
   if ((rc = collect_nodes(a0, &mv, g->nodes))) return g->fail(rc, a0->err);
-  g->plan.build(g->nodes, {{"parca_write_schema_version", "v2"}}, (int64_t)g->NT);
+  g->plan.build(g->nodes, {{"parca_write_schema_version", a0->cfg.schema == PA_SCHEMA_V1 ? "v1" : "v2"}}, (int64_t)g->NT);
   if (g->lz4 && (rc = merge_plan_lz4(g))) return rc;
   *ipc_len = g->lz4 ? g->lz.total : g->plan.total;
   g->planned = true;
@@ -969,6 +1160,11 @@ static void slice_of(const pa_merge* g, size_t i, uintptr_t tag, const void** pt
       *at = (uint64_t)mc.runbase * 4; *len = (uint64_t)mc.keep * 4;
       break;
     }
+    case SL_TS_RUNS: {
+      const MergeCol mc = g->cols_all[(size_t)me * g->ncols + col];
+      *ptr = a->v1_ts_vals; *at = (uint64_t)mc.runbase * 8; *len = (uint64_t)mc.keep * 8;
+      break;
+    }
     default: break;  // SL_VALID is assembled bit-wise (below)
   }
 }
@@ -1005,6 +1201,7 @@ static int merge_plan_lz4(pa_merge* g) {
       case SL_STOFF: case SL_STSIZE: return {rb * 4, n * 4};
       case SL_STREAM: return {(uint64_t)ctl_all[r].off0 * 4, (uint64_t)ctl_all[r].slice_len * 4};
       case SL_RUN_ENDS: case SL_RUN_KEYS: { const MergeCol mc = g->cols_all[(size_t)r * ncols + col]; return {(uint64_t)mc.runbase * 4, (uint64_t)mc.keep * 4}; }
+      case SL_TS_RUNS: { const MergeCol mc = g->cols_all[(size_t)r * ncols + col]; return {(uint64_t)mc.runbase * 8, (uint64_t)mc.keep * 8}; }
       case SL_VALID: {
         const MergeCol mc = g->cols_all[(size_t)r * ncols + col];
         const uint64_t b0 = ((uint64_t)mc.runbase + 7) / 8, b1 = ((uint64_t)mc.runbase + mc.keep + 7) / 8;
@@ -1356,6 +1553,55 @@ static int merge_collect(pa_merge* g, uint8_t* base, uint64_t cap, pa_agg_result
   return merge_result(g, base, root, total, t0, d2h, res, done);
 }
 
+// v1 groups: the stacktrace record for rank 0's request, built by every member from its copy of the store (the request's Gets
+// refresh every copy alike). Groups with one member per process first carry the request to every rank: its length in a small
+// all-gather, then rank 0's ids in an all-gather-v.
+static int merge_stacktraces(pa_merge* g, const uint8_t* ids, uint64_t n, pa_agg_result* res) {
+  memset(res, 0, sizeof *res);
+  const size_t L = g->members.size();
+  const uint32_t W = g->world;
+  if (g->members[0]->cfg.schema != PA_SCHEMA_V1) return g->fail(PA_EINVAL, "pa_merge_stacktraces needs a group of PA_SCHEMA_V1 members");
+  if (g->processed || g->planned) return g->fail(PA_EINVAL, "collect the merged batch before asking for stacktraces");
+  std::vector<uint8_t> req;
+  const uint8_t* use = ids;
+  if (L != W) {
+    const bool root = g->ranks[0] == 0;
+    const uint64_t kBad = ~0ull;  // rank 0's request is malformed: every rank fails, none waits for ids that never come
+    const uint64_t mine = !root ? 0 : (n && !ids) || n > 0x7FFFFFFFull / 16 ? kBad : n;
+    pa_agg* a = g->members[0];
+    MCK(cudaSetDevice(a->device));
+    MergeBufs& mb = g->mb[0];
+    MCK(mb.gather_scratch.ensure(std::max<size_t>((size_t)(W + 1) * 8, 256)));
+    uint8_t* slot = mb.gather_scratch.as<uint8_t>() + (size_t)W * 8;  // staged behind the gathered block
+    MCK(cudaMemcpyAsync(slot, &mine, 8, cudaMemcpyHostToDevice, a->s_comp));
+    MCK(cudaStreamSynchronize(a->s_comp));
+    std::vector<uint8_t> hn;
+    int rc = t_allgather_host(g, {slot}, 8, hn);
+    if (rc) return rc;
+    uint64_t n0;
+    memcpy(&n0, hn.data(), 8);  // rank 0's
+    if (n0 == kBad) return g->fail(PA_EINVAL, "rank 0's stacktrace request is malformed (null ids or more than int32 offsets allow)");
+    n = n0;
+    req.resize(n * 16);
+    if (n) {
+      MCK(mb.v1_ids_req.ensure(n * 16));
+      if (root) MCK(cudaMemcpyAsync(mb.v1_ids_req.p, ids, n * 16, cudaMemcpyHostToDevice, a->s_comp));
+      std::vector<uint64_t> count(W, 0), displ(W, 0);
+      count[0] = n * 16;
+      if ((rc = t_allgatherv(g, {mb.v1_ids_req.p}, {mb.v1_ids_req.p}, count, displ))) return rc;
+      MCK(cudaMemcpyAsync(req.data(), mb.v1_ids_req.p, n * 16, cudaMemcpyDeviceToHost, a->s_comp));
+      MCK(cudaStreamSynchronize(a->s_comp));
+    }
+    use = req.data();
+  }
+  for (size_t i = 0; i < L; i++) {
+    pa_agg_result mine{};
+    pa_agg* a = g->members[i];
+    if (int rc = stacktraces(a, use, n, i == 0 ? res : &mine)) return g->fail(rc, a->err);
+  }
+  return PA_OK;
+}
+
 }  // namespace pa
 
 
@@ -1372,6 +1618,15 @@ int pa_merge_create_local(pa_agg* const* members, uint32_t n, pa_merge** out) {
   if (n_lz4 && n_lz4 != n) {  // the reason goes where the caller of a PA_IPC_LZ4_FRAME_GPU member looks for it
     for (uint32_t i = 0; i < n; i++) if (lz4_gpu_member(members[i])) members[i]->fail(PA_EINVAL, kLz4Mixed);
     return PA_EINVAL;
+  }
+  for (uint32_t i = 1; i < n; i++) {  // (the reason goes into every member's last error)
+    const pa_agg *a = members[i], *b = members[0];
+    const char* why = a->cfg.schema != b->cfg.schema ? kSchemaMixed
+                    : (b->cfg.schema == PA_SCHEMA_V1 && (a->store_entries != b->store_entries || a->store_frames != b->store_frames)) ? kStoreMismatch : nullptr;
+    if (why) {
+      for (uint32_t j = 0; j < n; j++) members[j]->fail(PA_EINVAL, why);
+      return PA_EINVAL;
+    }
   }
   pa_merge* g = new pa_merge();
   g->world = n;
@@ -1536,6 +1791,11 @@ int pa_merge_flush(pa_merge* g, pa_agg_result* out) {
   if ((rc = merge_plan(g, &len))) { drop(); return rc; }
   if ((rc = merge_collect(g, nullptr, 0, out))) drop();
   return rc;
+}
+int pa_merge_stacktraces(pa_merge* g, const uint8_t* ids, uint64_t n_ids, pa_agg_result* out) {
+  if (!g || !out) return PA_EINVAL;
+  MergeLocks lk(g);
+  return merge_stacktraces(g, ids, n_ids, out);
 }
 int pa_merge_last_stats(const pa_merge* g, double* wall_ms, double* exchange_wait_ms, uint64_t* nvlink_bytes, uint64_t* n_rows_total) {
   if (!g) return PA_EINVAL;

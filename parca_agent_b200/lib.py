@@ -21,6 +21,7 @@ EXPORTS = [
     "pa_agg_debug_stack_ids", "pa_agg_debug_stack_counts", "pa_agg_debug_pair_counts", "pa_agg_stacktraces", "pa_agg_last_stack_ids", "pa_agg_shard_sizes", "pa_agg_shard_export", "pa_agg_stage_device", "pa_agg_stage_device_parts", "pa_agg_discard", "pa_ipc_compress_lz4", "pa_ipc_free", "pa_fix_truncation", "pa_xxh64",
     "pa_merge_create_local", "pa_merge_nccl_unique_id", "pa_merge_create_nccl", "pa_merge_destroy", "pa_merge_last_error", "pa_merge_process",
     "pa_merge_plan", "pa_merge_collect", "pa_merge_flush", "pa_merge_last_stats", "pa_merge_create_host", "pa_merge_create_shm",
+    "pa_merge_stacktraces",
 ]
 
 
@@ -88,6 +89,7 @@ def lib():
         L.pa_merge_collect.argtypes = [vp, vp, C.c_uint64, C.POINTER(abi.PaAggResult)]
         L.pa_merge_flush.argtypes = [vp, C.POINTER(abi.PaAggResult)]
         L.pa_merge_last_stats.argtypes = [vp, C.POINTER(C.c_double), C.POINTER(C.c_double), u64p, u64p]
+        L.pa_merge_stacktraces.argtypes = [vp, C.c_char_p, C.c_uint64, C.POINTER(abi.PaAggResult)]
         _LIB = L
     return _LIB
 
@@ -340,6 +342,15 @@ class MergeGroup:
     def flush(self):
         raw = abi.PaAggResult()
         self._ck(lib().pa_merge_flush(self.h, C.byref(raw)))
+        return Result(raw)
+
+    def stacktraces(self, ids=None):
+        """v1 groups (collective): the stacktrace record for rank 0's concatenated 16-byte ids; other ranks pass None. Every rank
+        gets its own member's record (the same bytes everywhere), valid until that member's next flush or request."""
+        ids = b"" if ids is None else bytes(ids)
+        assert len(ids) % 16 == 0
+        raw = abi.PaAggResult()
+        self._ck(lib().pa_merge_stacktraces(self.h, ids or None, len(ids) // 16, C.byref(raw)))
         return Result(raw)
 
     def stats(self):

@@ -6,7 +6,9 @@ usage: PA_EARLY_D2H_ALWAYS=1 compute-sanitizer --tool memcheck python tools/sani
 lz4_gpu: small flushes with the bodies compressed on the device (PA_IPC_LZ4_FRAME_GPU) instead: a multi-chunk v2 batch, the
 narrow ring, and a v1 batch with its stacktrace record, each checked against the oracle's plain stream.
 merge_lz4_gpu: a small in-process merge group of PA_IPC_LZ4_FRAME_GPU members whose shard cuts put blocks across part borders
-(heads exchange, crossing blocks, an empty shard), checked against one such aggregator on the concatenated rows."""
+(heads exchange, crossing blocks, an empty shard), checked against one such aggregator on the concatenated rows.
+merge_v1: in-process groups of PA_SCHEMA_V1 members over several intervals against a small store (evictions, compaction, an
+over-full batch, stacktrace requests), plain and PA_IPC_LZ4_FRAME_GPU, checked against one v1 aggregator and the oracle."""
 import os
 import sys
 
@@ -65,12 +67,21 @@ def merge_lz4_gpu():
     print("sanitize_small merge_lz4_gpu ok")
 
 
+def merge_v1():
+    from test_merge_v1 import lru_scenario
+    lru_scenario(oracle_py, lib, 3, intervals=6).close()
+    lru_scenario(oracle_py, lib, 2, lz4=True, intervals=4).close()
+    print("sanitize_small merge_v1 ok")
+
+
 def main():
     oracle_py.build()
     if sys.argv[1:] == ["lz4_gpu"]:
         return lz4_gpu()
     if sys.argv[1:] == ["merge_lz4_gpu"]:
         return merge_lz4_gpu()
+    if sys.argv[1:] == ["merge_v1"]:
+        return merge_v1()
     # early copy-out: several intervals through one aggregator, 7 chunks each
     base = synth.edge_workload(seed=3, n=3000, hash_mode=abi.PA_HASH_XXH64X2, external=False)
     for kw in ({}, {"frame_id_bytes": 4}):
