@@ -81,6 +81,16 @@ enum {
 
 #define PA_CFG_SINGLE_RING 0x1u /* one ring buffer instead of two: ingest is refused (PA_ENOSPC) while a flush holds the ring.
                                     Halves the pinned host memory; for replay / batch use, not for a live agent */
+#define PA_CFG_REGISTERED_STACKS 0x2u /* registered stacks: stacks are registered once (pa_agg_register_stacks) and a sample row
+                                    names its stack by id in frame_off; the ring holds 64-byte headers only (no frame ids, no frame
+                                    ring, no device frame buffer). Works with both hash modes, both schemas, both frame_id_bytes and
+                                    every ipc_compression; the output is byte for byte the record of the same rows with their frame ids
+                                    in the ring. Row meaning in this mode: frame_off = a registered stack id; hash_hi / hash_lo and
+                                    nframes are ignored (the stack's registration supplies them); pa_agg_acquire takes n_frames == 0
+                                    and hands out *frames = NULL; pa_agg_submit ignores `frames` and keeps the caller's frame_off. A row
+                                    whose stack id is not registered fails the flush with PA_EINVAL (the next flush works).
+                                    max_frames (0 = max_samples * 64) bounds the registered frames instead of the ring.
+                                    Not supported yet (PA_EINVAL): pa_merge_create_*, pa_agg_shard_export, pa_agg_stage_device(_parts) */
 
 #define PA_NO_STRING 0xFFFFFFFFu /* "no value"; string id 0 is always the empty string "" */
 
@@ -95,7 +105,8 @@ typedef struct pa_sample_hdr {
   uint32_t comm_sid;     /* string id of meta.Comm → label thread_name (:624); 0 (= "") drops it */
   uint32_t labelset_id;  /* per-PID cached labels (content of the labels LRU, :569) */
   uint64_t frame_off;    /* index of this sample's first frame id in the batch frame stream;
-                            filled by pa_agg_submit / by the producer after pa_agg_acquire */
+                            filled by pa_agg_submit / by the producer after pa_agg_acquire.
+                            PA_CFG_REGISTERED_STACKS: the registered stack id of this sample (set by the caller) */
   uint32_t cpu;          /* meta.CPU → label cpu (:618) */
   uint16_t nframes;      /* len(trace.Frames) */
   uint8_t kind;          /* PA_KIND_* */
@@ -137,7 +148,7 @@ typedef struct pa_agg_config {
   uint32_t n_external_labels;  /* --metadata-external-labels → LabelAll at flush (:1760-1764) */
   const pa_label_pair* external_labels; /* string ids must be registered before the first flush */
   uint64_t max_samples;        /* ring capacity in rows (per buffer; two buffers are kept) */
-  uint64_t max_frames;         /* ring capacity in frame ids (per buffer) */
+  uint64_t max_frames;         /* ring capacity in frame ids (per buffer); PA_CFG_REGISTERED_STACKS: capacity of the registered frames */
   uint32_t chunk_samples;      /* H2D/compute overlap granularity; 0 = default */
   uint32_t schema;             /* PA_SCHEMA_V2 (0, default here) or PA_SCHEMA_V1 (--remote-store-use-v2-schema=false,
                                   flags/flags.go:349): which sample record pa_agg_flush builds */
@@ -197,6 +208,15 @@ int pa_agg_register_strings(pa_agg* a, const uint8_t* bytes, const uint32_t* off
 int pa_agg_register_frames(pa_agg* a, const pa_frame_desc* descs, uint32_t n, uint64_t* first_frame_id);
 /* labelsets: n sets, set i = pairs[offsets[i]..offsets[i+1]) sorted by name (labels.Labels order). */
 int pa_agg_register_labelsets(pa_agg* a, const pa_label_pair* pairs, const uint32_t* offsets, uint32_t n, uint32_t* first_id);
+/* stacks (PA_CFG_REGISTERED_STACKS only): n stacks, stack i = frames[offsets[i]..offsets[i+1]) (uint32 ids when
+ * frame_id_bytes = 4, as in pa_agg_submit); ids are dense and append-only like frame ids, *first_stack_id receives the first.
+ * hashes: 2n words hash_hi, hash_lo per stack, as in pa_sample_hdr; required in PA_HASH_PROVIDED mode and NULL in
+ * PA_HASH_XXH64X2 mode, where the library computes each id here with the definition the GPU uses for ring rows (XXH64 over the
+ * ids as little-endian uint64, seeds 0 and PA_XXH_SEED_LO; pa_xxh64). Thread-safe, may run during a flush; a batch uses the
+ * stacks registered when it is processed. All or nothing: a refused call registers no stack.
+ * PA_EINVAL: unregistered frame id, aggregator without the flag, hashes given / missing for the hash mode.
+ * PA_ERANGE: a stack deeper than 65535. PA_ENOSPC: the registered frames would exceed max_frames. */
+int pa_agg_register_stacks(pa_agg* a, const uint64_t* hashes, const uint64_t* frames, const uint64_t* offsets, uint32_t n, uint64_t* first_stack_id);
 
 /* ingest — ReportTraceEvent (:219). Thread-safe; row order == acquisition order (the mutex at :335).
  * acquire reserves space for n_rows headers / n_frames frame ids in the pinned ring and returns

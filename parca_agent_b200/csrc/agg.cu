@@ -106,9 +106,11 @@ struct MergeDims { uint32_t world = 1, rank = 0; uint64_t row_base = 0, n_total 
 struct Pass {
   // registration state as mirrored to the device for this batch (snapshot taken under reg_mu in upload_tables)
   uint32_t n_cstr = 0, n_frames = 0, n_funcs = 0, n_sids = 0, n_labelsets = 0;
+  uint32_t n_stacks = 0;          // registered stacks (PA_CFG_REGISTERED_STACKS)
+  uint64_t n_stack_frames = 0;    // and the frame ids of their arena
   uint64_t N = 0, NT = 0, row_base = 0;
   uint32_t world = 1, rank = 0, ncols = 0, nlab = 0;
-  bool v1 = false, provided = false, merged = false;
+  bool v1 = false, provided = false, merged = false;  // provided: the stack ids arrive with the rows (or their registered stacks)
   uint64_t cap = 0, tcap = 0;
   uint32_t mask = 0;
   size_t Pn = 1, S = 1, FN = 1, NI = 1;
@@ -181,6 +183,12 @@ struct pa_agg {
   Mirror<uint64_t> m_addr, m_line;
   Mirror<uint32_t> m_type, m_map, m_bid, m_func, m_fnfile, m_sid2cid;
   DBuf d_lsmat, d_kindtab, d_cols, d_jobs;
+  // PA_CFG_REGISTERED_STACKS: the registered stacks and their frame arena (ids at the ring's width, idb / 4 words each)
+  bool registered = false;
+  std::vector<RegStack> reg_stacks;
+  std::vector<uint32_t> reg_arena;
+  Mirror<RegStack> m_stacks;
+  Mirror<uint32_t> m_arena;
   // v1: frames resolved by the buildStacktraceRecord rules + the device-resident store of known stacks
   Mirror<uint32_t> m1_map, m1_bid, m1_fn, m1_file;
   Mirror<uint64_t> m1_line, m1_col;
@@ -388,6 +396,7 @@ int pa_agg_create(const pa_agg_config* cfg, pa_agg** out) {
   a->device = cfg->device;
   a->idb = cfg->frame_id_bytes == 4 ? 4u : 8u;
   a->single_ring = (cfg->flags & PA_CFG_SINGLE_RING) != 0;
+  a->registered = (cfg->flags & PA_CFG_REGISTERED_STACKS) != 0;
   auto bail = [&](int code) { pa_agg_destroy(a); return code; };
   if (cudaSetDevice(a->device) != cudaSuccess) return bail(PA_ENODEV);
   cudaDeviceProp prop;
@@ -454,6 +463,7 @@ int pa_agg_create(const pa_agg_config* cfg, pa_agg** out) {
   if (a->idb == 4 && a->hash_variant != 5) a->hash_variant = 2;  // (the tma variants fall through to wide32 in launch_hash)  // the narrow ring is read by the `wide` kernel (widening loads); the other variants take uint64 ids
   for (int r = 0; r < (a->single_ring ? 1 : 2); r++) {
     if (cudaHostAlloc((void**)&a->ring[r].hdr, N * sizeof(pa_sample_hdr), cudaHostAllocDefault) != cudaSuccess) return bail(PA_ENOMEM);
+    if (a->registered) continue;  // rows name registered stacks: the ring carries no frame ids
     if (cudaHostAlloc((void**)&a->ring[r].frames, std::max<uint64_t>(NF, 1) * a->idb + 64, cudaHostAllocMapped) != cudaSuccess) return bail(PA_ENOMEM);
     void* dp = nullptr;  // device alias of the pinned frame ring (provided-hash mode gathers unique stacks straight from it)
     if (cudaHostGetDevicePointer(&dp, a->ring[r].frames, 0) != cudaSuccess) return bail(PA_EIO);
@@ -463,7 +473,7 @@ int pa_agg_create(const pa_agg_config* cfg, pa_agg** out) {
   bool ok = true;
   auto need = [&](DBuf& b, uint64_t bytes) { ok = ok && b.ensure(std::max<uint64_t>(bytes, 256)) == cudaSuccess; };
   need(a->d_hdr, N * 64);
-  if (a->cfg.hash_mode == PA_HASH_XXH64X2) need(a->d_frames, NF * a->idb + 64);  // provided-hash mode never uploads the frame stream (+ slack: bulk copies round up to 16 B)
+  if (a->cfg.hash_mode == PA_HASH_XXH64X2 && !a->registered) need(a->d_frames, NF * a->idb + 64);  // provided-hash mode never uploads the frame stream (+ slack: bulk copies round up to 16 B)
   need(a->d_ts, N * 8); need(a->d_value, N * 8); need(a->d_uuid, N * 16); need(a->d_stoff, N * 4); need(a->d_stsize, N * 4);
   need(a->d_slot, N * 4); need(a->d_kind, N); need(a->d_nfr, N * 2); need(a->d_foff, N * 8);
   need(a->d_ls, N * 4); need(a->d_cpu, N * 4); need(a->d_tid, N * 4); need(a->d_comm, N * 4);
@@ -516,7 +526,7 @@ void pa_agg_destroy(pa_agg* a) {
   DBuf* all[] = {&a->d_hdr, &a->d_frames, &a->d_ts, &a->d_value, &a->d_uuid, &a->d_stoff, &a->d_stsize, &a->d_slot, &a->d_kind, &a->d_nfr,
                  &a->d_foff, &a->d_ls, &a->d_cpu, &a->d_tid, &a->d_comm, &a->d_ustream, &a->d_uniq_row, &a->d_uniq_count, &a->d_table, &a->d_ctr,
                  &a->d_arena, &a->d_partial, &a->d_partial2, &a->d_ree_partial, &a->d_lsmat, &a->d_kindtab, &a->d_cols, &a->d_jobs,
-                 &a->m_addr.buf, &a->m_line.buf, &a->m_type.buf, &a->m_map.buf, &a->m_bid.buf, &a->m_func.buf, &a->m_fnfile.buf, &a->m_sid2cid.buf,
+                 &a->m_stacks.buf, &a->m_arena.buf, &a->m_addr.buf, &a->m_line.buf, &a->m_type.buf, &a->m_map.buf, &a->m_bid.buf, &a->m_func.buf, &a->m_fnfile.buf, &a->m_sid2cid.buf,
                  &a->m1_map.buf, &a->m1_bid.buf, &a->m1_fn.buf, &a->m1_file.buf, &a->m1_line.buf, &a->m1_col.buf, &a->m1_complete.buf,
                  &a->d_store, &a->d_store_arena, &a->d_store_ctl, &a->d_v1_ids, &a->d_st1, &a->d_store_stamp, &a->d_v1_last, &a->d_select, &a->d_lz4, &a->d_lz4_body};
   for (DBuf* b : all) b->release();
@@ -574,16 +584,64 @@ int pa_agg_register_labelsets(pa_agg* a, const pa_label_pair* pairs, const uint3
   a->cols_dirty = true;
   return PA_OK;
 }
+int pa_agg_register_stacks(pa_agg* a, const uint64_t* hashes, const uint64_t* frames, const uint64_t* offsets, uint32_t n, uint64_t* first_stack_id) {
+  if (!a) return PA_EINVAL;
+  if (!a->registered) return a->fail(PA_EINVAL, "pa_agg_register_stacks needs an aggregator created with PA_CFG_REGISTERED_STACKS");
+  if (n && !offsets) return PA_EINVAL;
+  const bool provided = a->cfg.hash_mode == PA_HASH_PROVIDED;
+  if (n && provided && !hashes) return a->fail(PA_EINVAL, "PA_HASH_PROVIDED: register_stacks needs the stack ids (hashes)");
+  if (!provided && hashes) return a->fail(PA_EINVAL, "PA_HASH_XXH64X2: the library computes the stack ids (hashes must be NULL)");
+  std::lock_guard<std::mutex> g(a->reg_mu);
+  const uint64_t nf_reg = a->ft.count(), words = a->idb / 4;
+  const uint64_t have = a->reg_arena.size() / words;
+  uint64_t total = 0;
+  for (uint32_t i = 0; i < n; i++) {  // validate everything first: a refused call registers nothing
+    if (offsets[i + 1] < offsets[i]) return a->fail(PA_EINVAL, "stack offsets must be non-decreasing");
+    const uint64_t d = offsets[i + 1] - offsets[i];
+    if (d > 0xFFFFu) return a->fail(PA_ERANGE, "stack deeper than 65535 frames");
+    total += d;
+  }
+  if (total && !frames) return PA_EINVAL;
+  if (have + total > a->cfg.max_frames) return a->fail(PA_ENOSPC, "registered frames would exceed max_frames");
+  if (a->reg_stacks.size() + n > 0xFFFFFFFFull) return a->fail(PA_ENOSPC, "more than 2^32 - 1 registered stacks");  // (ids are checked as uint32 on the device)
+  const uint32_t* f32 = (const uint32_t*)frames;
+  for (uint32_t i = 0; i < n; i++)
+    for (uint64_t j = offsets[i]; j < offsets[i + 1]; j++)
+      if ((a->idb == 4 ? (uint64_t)f32[j] : frames[j]) >= nf_reg) return a->fail(PA_EINVAL, "stack refers to an unregistered frame id");
+  if (first_stack_id) *first_stack_id = a->reg_stacks.size();
+  std::vector<uint64_t> wide;
+  for (uint32_t i = 0; i < n; i++) {
+    const uint64_t d = offsets[i + 1] - offsets[i];
+    RegStack s{};
+    s.off = a->reg_arena.size() / words;
+    s.depth = (uint32_t)d;
+    const uint8_t* src = (const uint8_t*)frames + offsets[i] * a->idb;
+    a->reg_arena.resize(a->reg_arena.size() + d * words);
+    if (d) memcpy(a->reg_arena.data() + s.off * words, src, d * a->idb);
+    if (provided) {
+      s.hash_hi = hashes[2 * i];
+      s.hash_lo = hashes[2 * i + 1];
+    } else {  // the stack id of a ring row with these frames (DESIGN section 3): XXH64 over the ids as little-endian uint64
+      wide.resize(d);
+      for (uint64_t j = 0; j < d; j++) wide[j] = a->idb == 4 ? (uint64_t)f32[offsets[i] + j] : frames[offsets[i] + j];
+      s.hash_hi = pa_xxh64(wide.data(), d * 8, 0);
+      s.hash_lo = pa_xxh64(wide.data(), d * 8, PA_XXH_SEED_LO);
+    }
+    a->reg_stacks.push_back(s);
+  }
+  return PA_OK;
+}
 
 // ---- ingest ----------------------------------------------------------------------------------
 int pa_agg_acquire(pa_agg* a, uint64_t n_rows, uint64_t n_frames, pa_sample_hdr** hdrs, uint64_t** frames, uint64_t* frame_base) {
   if (!a || !hdrs || !frames) return PA_EINVAL;
+  if (a->registered && n_frames) return PA_EINVAL;  // rows name registered stacks (ingest may be concurrent: no error text)
   std::lock_guard<std::mutex> g(a->ring_mu);
   if (a->ring_busy) return PA_ENOSPC;  // single ring: a flush holds the buffer
   pa_agg::Ring& r = a->ring[a->active];
   if (n_rows > a->cfg.max_samples || n_frames > a->cfg.max_frames || r.rows + n_rows > a->cfg.max_samples || r.nfr + n_frames > a->cfg.max_frames) return PA_ENOSPC;
   *hdrs = r.hdr + r.rows;
-  *frames = (uint64_t*)((uint8_t*)r.frames + r.nfr * a->idb);  // uint32 ids when the ring is narrow
+  *frames = a->registered ? nullptr : (uint64_t*)((uint8_t*)r.frames + r.nfr * a->idb);  // uint32 ids when the ring is narrow
   if (frame_base) *frame_base = r.nfr;
   r.rows += n_rows;
   r.nfr += n_frames;
@@ -599,6 +657,13 @@ int pa_agg_commit(pa_agg* a, uint64_t) {
 }
 int pa_agg_submit(pa_agg* a, const pa_sample_hdr* hdrs, const uint64_t* frames, uint64_t n_rows) {
   if (!a || (n_rows && !hdrs)) return PA_EINVAL;
+  if (a->registered) {  // frame_off is the caller's stack id: copied as it is
+    pa_sample_hdr* dh; uint64_t* df; uint64_t base;
+    int rc = pa_agg_acquire(a, n_rows, 0, &dh, &df, &base);
+    if (rc) return rc;
+    if (n_rows) memcpy(dh, hdrs, n_rows * sizeof(pa_sample_hdr));
+    return pa_agg_commit(a, n_rows);
+  }
   uint64_t nf = 0;
   for (uint64_t i = 0; i < n_rows; i++) nf += hdrs[i].nframes;
   if (nf && !frames) return PA_EINVAL;
@@ -638,7 +703,8 @@ static int stage_async(pa_agg* a) {
   }
   pa_agg::Ring& r = a->ring[buf];
   a->staged = buf;
-  a->src_frames = a->cfg.hash_mode == PA_HASH_PROVIDED ? (const unsigned long long*)r.frames_dev : a->d_frames.as<unsigned long long>();
+  // (registered stacks: the device arena, set by upload_tables once the batch's registrations are mirrored)
+  a->src_frames = a->registered ? nullptr : a->cfg.hash_mode == PA_HASH_PROVIDED ? (const unsigned long long*)r.frames_dev : a->d_frames.as<unsigned long long>();
   a->N = r.rows;
   a->NF = r.nfr;
   a->processed = false;
@@ -653,7 +719,8 @@ static int stage_async(pa_agg* a) {
   // headers first when the frame ids take several chunks: everything that depends only on the headers (k_header, the label chain,
   // the early copy-out) then overlaps the upload of the ids
   // (the compressed stream's layout is only known once its bodies are encoded: PA_IPC_LZ4_FRAME_GPU has no early copy-out)
-  a->early.hdr_first = a->early_enabled && a->cfg.ipc_compression != PA_IPC_LZ4_FRAME_GPU && nchunks > 1 && a->cfg.hash_mode == PA_HASH_XXH64X2 && a->cfg.schema != PA_SCHEMA_V1 && !a->serial;
+  const bool upload_ids = a->cfg.hash_mode == PA_HASH_XXH64X2 && !a->registered;
+  a->early.hdr_first = a->early_enabled && a->cfg.ipc_compression != PA_IPC_LZ4_FRAME_GPU && nchunks > 1 && upload_ids && a->cfg.schema != PA_SCHEMA_V1 && !a->serial;
   if (a->early.hdr_first) {
     CK(cudaMemcpyAsync(a->d_hdr.p, r.hdr, a->N * 64, cudaMemcpyHostToDevice, a->s_copy));
     CK(cudaEventRecord(a->ev_hdr_all, a->s_copy));
@@ -663,13 +730,14 @@ static int stage_async(pa_agg* a) {
   for (uint64_t k = 0; k < nchunks; k++) {
     uint64_t r0 = k * C, r1 = std::min(a->N, r0 + C);
     // frames are laid out in row order (acquire hands out ascending frame_base): a chunk's frames end where the next chunk's begin
-    uint64_t fend = (r1 < a->N) ? std::min<uint64_t>(r.hdr[r1].frame_off, a->NF) : a->NF;
+    uint64_t fend = (r1 < a->N && !a->registered) ? std::min<uint64_t>(r.hdr[r1].frame_off, a->NF) : a->NF;
     if (fend < fdone) fend = fdone;
     if (!a->early.hdr_first) CK(cudaMemcpyAsync(a->d_hdr.as<uint8_t>() + r0 * 64, r.hdr + r0, (r1 - r0) * 64, cudaMemcpyHostToDevice, a->s_copy));
     // The stack id arrives with the sample in PA_HASH_PROVIDED mode (the reference's dataflow, parca_reporter.go:224):
     // frames are only needed for each stack's FIRST occurrence, so nothing is uploaded here and k_gather_unique
     // reads those few stacks from the mapped pinned ring over PCIe (U*F*8 bytes instead of N*F*8).
-    if (fend > fdone && a->cfg.hash_mode == PA_HASH_XXH64X2)
+    // Registered stacks: the ring holds headers only; the frames are in the device arena already.
+    if (fend > fdone && upload_ids)
       CK(cudaMemcpyAsync(a->d_frames.as<uint8_t>() + fdone * a->idb, (const uint8_t*)r.frames + fdone * a->idb, (fend - fdone) * a->idb, cudaMemcpyHostToDevice,
                          (a->s_copy2 && a->early.hdr_first && (k & 1)) ? a->s_copy2 : a->s_copy));
     fdone = fend;
@@ -727,6 +795,11 @@ static int upload_tables(pa_agg* a) {
     CK(a->m1_map.sync(a->ft.v1_map_cid, s)); CK(a->m1_bid.sync(a->ft.v1_bid_cid, s)); CK(a->m1_fn.sync(a->ft.v1_fn_cid, s));
     CK(a->m1_file.sync(a->ft.v1_file_cid, s)); CK(a->m1_line.sync(a->ft.v1_line, s)); CK(a->m1_col.sync(a->ft.v1_col, s));
     CK(a->m1_complete.sync(a->ft.v1_complete, s));
+  }
+  if (a->registered) {
+    CK(a->m_stacks.sync(a->reg_stacks, s)); CK(a->m_arena.sync(a->reg_arena, s));
+    a->src_frames = (const unsigned long long*)a->m_arena.ptr();  // (a regrown mirror moves: set on every upload)
+    a->P.n_stacks = (uint32_t)a->reg_stacks.size(); a->P.n_stack_frames = a->reg_arena.size() / (a->idb / 4);
   }
   // what the device mirrors now hold: the pass uses these counts only (registration may continue concurrently)
   a->P.n_cstr = a->sp.count(); a->P.n_frames = a->ft.count(); a->P.n_funcs = a->ft.n_funcs();
@@ -931,7 +1004,7 @@ static int pass_plan(pa_agg* a, const MergeDims* md) {
   P.ncols = (uint32_t)a->cols.size();
   P.nlab = a->n_label_cols;
   P.v1 = a->cfg.schema == PA_SCHEMA_V1;
-  P.provided = a->cfg.hash_mode == PA_HASH_PROVIDED;
+  P.provided = a->cfg.hash_mode == PA_HASH_PROVIDED || a->registered;
   const uint32_t ncols = P.ncols, nlab = P.nlab;
   const bool v1 = P.v1;
 
@@ -958,7 +1031,8 @@ static int pass_plan(pa_agg* a, const MergeDims* md) {
   std::vector<Req> reqs;
   auto want = [&reqs](auto** pp, size_t bytes, int cls = 2) { reqs.push_back(Req{(void**)pp, (bytes + 255) & ~(size_t)255, cls}); };
   const size_t Pn = std::max<uint32_t>(P.n_frames, 1), S = std::max<uint32_t>(P.n_cstr, 1), FN = std::max<uint32_t>(P.n_funcs, 1);
-  const uint64_t nf_all = md ? md->nf_total : a->NF;
+  // (registered stacks: the unique stacks' frames are a subset of the arena's, as in the ring they are of the batch's)
+  const uint64_t nf_all = md ? md->nf_total : a->registered ? P.n_stack_frames : a->NF;
   const size_t NI = (size_t)std::min<uint64_t>(std::max<uint64_t>(nf_all, 1), 0x7FFFFFFFull);
   const size_t Nn = (size_t)std::max<uint64_t>(N, 1), NTn = (size_t)std::max<uint64_t>(P.NT, 1);
   P.Pn = Pn; P.S = S; P.FN = FN; P.NI = NI;
@@ -1142,9 +1216,11 @@ static int pass_front(pa_agg* a) {
       if (a->cols[c].type == COL_COMM) h.first_comm = P.col_first[c];
     }
     h.first_kind = P.v1 ? a->v1_first_kind : nullptr;
+    h.stacks = (const uint4*)a->m_stacks.ptr(); h.n_stacks = P.n_stacks;
     uint64_t rows = r1 - r0;
     int hb = (int)std::min<uint64_t>((rows + kThreads - 1) / kThreads, (uint64_t)a->sms * kHdrBlocksPerSm);
-    k_header<<<std::max(hb, 1), kThreads, 0, s>>>(h);
+    if (a->registered) k_header<true><<<std::max(hb, 1), kThreads, 0, s>>>(h);
+    else k_header<false><<<std::max(hb, 1), kThreads, 0, s>>>(h);
     a->tm[T_HEADER].launches++;
   };
   auto launch_hash = [&](uint64_t r0, uint64_t r1) {
@@ -1403,6 +1479,7 @@ static int check_batch_errors(pa_agg* a, uint32_t e) {
   if (e & ERR_BAD_FRAME_RANGE) return a->fail(PA_EINVAL, "sample frame range outside the staged frames (frame_off must ascend with the rows)");
   if (e & ERR_SLICE_CAP) return a->fail(PA_ENOSPC, "merged batch: this shard's part of the location-index stream exceeds max_frames");
   if (e & ERR_MERGE_LOOKUP) return a->fail(PA_EIO, "merged batch: a local stack is missing from the merged dictionary");
+  if (e & ERR_BAD_STACK_ID) return a->fail(PA_EINVAL, "sample refers to an unregistered stack id (PA_CFG_REGISTERED_STACKS: frame_off is a stack id)");
   return PA_OK;
 }
 
@@ -2441,7 +2518,9 @@ static int stacktraces(pa_agg* a, const uint8_t* ids, uint64_t n, pa_agg_result*
 
 // ---------------------------------------------------------------------------------------------
 // mode B building blocks (see include/parcaagg.h): export a processed shard, stage a merged batch from device memory
+static const char kRegisteredUnsupported[] = "not supported with PA_CFG_REGISTERED_STACKS (rows name registered stacks, not frame ranges)";
 static int stage_device(pa_agg* a, const pa_sample_hdr* hdr, uint64_t n_rows, const uint64_t* frames, uint64_t n_frames) {
+  if (a->registered) return a->fail(PA_EINVAL, kRegisteredUnsupported);
   CK(cudaSetDevice(a->device));
   if (a->staged >= 0) return a->fail(PA_EINVAL, "the previously staged batch has not been collected");
   if (n_rows > a->cfg.max_samples || n_frames > a->cfg.max_frames) return a->fail(PA_ENOSPC, "device batch exceeds max_samples / max_frames");
@@ -2464,6 +2543,7 @@ static int stage_device(pa_agg* a, const pa_sample_hdr* hdr, uint64_t n_rows, co
 }
 
 static int stage_device_parts(pa_agg* a, const pa_device_part* parts, uint32_t n_parts, uint64_t n_total) {
+  if (a->registered) return a->fail(PA_EINVAL, kRegisteredUnsupported);
   CK(cudaSetDevice(a->device));
   if (a->staged >= 0) return a->fail(PA_EINVAL, "the previously staged batch has not been collected");
   if (n_parts && !parts) return a->fail(PA_EINVAL, "null parts");
@@ -2507,6 +2587,7 @@ static int stage_device_parts(pa_agg* a, const pa_device_part* parts, uint32_t n
 }
 
 static int shard_export(pa_agg* a, uint64_t frame_base, pa_sample_hdr* hdr_out, uint64_t* frames_out) {
+  if (a->registered) return a->fail(PA_EINVAL, kRegisteredUnsupported);
   if (a->cfg.schema != PA_SCHEMA_V2) return a->fail(PA_EINVAL, "shard export needs a PA_SCHEMA_V2 aggregator (the v2 pipeline gathers the unique stacks)");
   if (a->staged < 0 || !a->processed) return a->fail(PA_EINVAL, "shard export needs a processed, not yet collected batch");
   if (!a->N) return PA_OK;

@@ -23,9 +23,18 @@ enum : uint32_t {
   ERR_BAD_KIND = 16u, ERR_INDEX_OVERFLOW = 32u, ERR_BAD_CPU = 64u, ERR_BAD_FRAME_RANGE = 128u,
   ERR_SLICE_CAP = 256u,   // mode B: this shard's slice of the location-index stream exceeds its buffer
   ERR_MERGE_LOOKUP = 512u,  // mode B: a local stack is missing from the merged dictionary (internal error)
+  ERR_BAD_STACK_ID = 1024u, // registered stacks: a row names a stack id that was not registered when the batch was processed
 };
 
 struct __align__(16) Key128 { unsigned long long hi, lo; };
+
+// PA_CFG_REGISTERED_STACKS: one registered stack, 32 B (one L2 sector). `off` indexes the registered frame arena, which holds
+// the ids at the ring's width, so every kernel that reads frames through (frames, frame_off, narrow) reads the arena unchanged.
+struct __align__(32) RegStack {
+  unsigned long long hash_hi, hash_lo;  // the stack id, as pa_sample_hdr carries it
+  unsigned long long off;
+  uint32_t depth, pad;
+};
 
 // open-address stack table entry: 32 B = one L2 sector
 struct __align__(32) StackSlot {
@@ -262,6 +271,8 @@ struct HeaderArgs {
   uint32_t tid_mask;
   uint32_t* first_comm;
   uint32_t* first_kind;          // [8] first row of each sample kind (v1: the kind-derived columns are dictionary encoded)
+  const uint4* stacks;           // k_header<true>: the registered stack records (RegStack, two uint4 each)
+  uint32_t n_stacks;             // records mirrored for this batch
 };
 
 // Each warp works through tiles of 32 consecutive rows (2 KB of contiguous headers). The next tile's headers arrive in the
@@ -271,8 +282,11 @@ struct HeaderArgs {
 // 2 KB of shared memory and at most 32 registers per thread keep all 64 warps of an SM resident, as many as these
 // latency-bound lookups want. The shared-memory carveout is left to the driver: the rest of L1 caches the small lookup
 // tables, and forcing the largest carveout made the pass about 30 % slower in provided-hash mode on an H100.
+// kRegistered (PA_CFG_REGISTERED_STACKS): frame_off names a registered stack; its 32-byte record supplies the stack id, the
+// depth and the arena offset, and hash_hi / hash_lo / nframes of the row are ignored. Launched with provided = 1.
 constexpr int kHdrBlocksPerSm = 8;
 
+template <bool kRegistered>
 __global__ void __launch_bounds__(kThreads, kHdrBlocksPerSm) k_header(HeaderArgs a) {
   __shared__ __align__(128) uint4 tile_buf[kWarps][32 * 4];
   __shared__ __align__(8) unsigned long long tile_bar[kWarps];
@@ -326,7 +340,17 @@ __global__ void __launch_bounds__(kThreads, kHdrBlocksPerSm) k_header(HeaderArgs
       if (ls >= a.n_labelsets) { err |= ERR_BAD_LABELSET; ls = 0; }
       if (comm_sid >= a.n_sids) { err |= ERR_BAD_STRING_ID; comm_sid = 0; }
       if (cpu >= 65536u) { err |= ERR_BAD_CPU; cpu = 0; }
-      if (foff + nfr > a.n_frame_ids) { err |= ERR_BAD_FRAME_RANGE; nfr = 0; foff = 0; }
+      if (kRegistered) {
+        if (foff < a.n_stacks) {
+          const uint4 s0 = __ldg(a.stacks + 2 * foff), s1 = __ldg(a.stacks + 2 * foff + 1);
+          k.hi = ((unsigned long long)s0.y << 32) | s0.x;
+          k.lo = ((unsigned long long)s0.w << 32) | s0.z;
+          foff = ((unsigned long long)s1.y << 32) | s1.x;
+          nfr = s1.z;
+        } else {
+          err |= ERR_BAD_STACK_ID; k = Key128{0ull, 0ull}; nfr = 0; foff = 0;
+        }
+      } else if (foff + nfr > a.n_frame_ids) { err |= ERR_BAD_FRAME_RANGE; nfr = 0; foff = 0; }
       if (err) atomicOr(&a.ctr->err, err);
       a.timestamp[r] = ts;
       a.value[r] = (knd == 0) ? 1ll : val;  // TraceOriginSampling writes value 1 (:340)

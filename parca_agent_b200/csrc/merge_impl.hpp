@@ -1608,6 +1608,13 @@ static int merge_stacktraces(pa_merge* g, const uint8_t* ids, uint64_t n, pa_agg
 // ---------------------------------------------------------------------------------------------------------------------
 extern "C" {
 
+// registered-stacks members are not supported by merge groups yet (the reason goes into the member's last error)
+static bool refuse_registered(pa_agg* m) {
+  if (!m->registered) return false;
+  m->fail(PA_EINVAL, "merge groups do not support PA_CFG_REGISTERED_STACKS members yet");
+  return true;
+}
+
 int pa_merge_create_local(pa_agg* const* members, uint32_t n, pa_merge** out) {
   if (!members || !n || !out || n > (uint32_t)kMaxWorld) return PA_EINVAL;
   uint32_t n_lz4 = 0;
@@ -1615,6 +1622,9 @@ int pa_merge_create_local(pa_agg* const* members, uint32_t n, pa_merge** out) {
     if (!members[i] || members[i]->device != members[0]->device) return PA_EINVAL;
     n_lz4 += lz4_gpu_member(members[i]);
   }
+  bool any_registered = false;
+  for (uint32_t i = 0; i < n; i++) any_registered |= refuse_registered(members[i]);
+  if (any_registered) return PA_EINVAL;
   if (n_lz4 && n_lz4 != n) {  // the reason goes where the caller of a PA_IPC_LZ4_FRAME_GPU member looks for it
     for (uint32_t i = 0; i < n; i++) if (lz4_gpu_member(members[i])) members[i]->fail(PA_EINVAL, kLz4Mixed);
     return PA_EINVAL;
@@ -1647,6 +1657,7 @@ int pa_merge_nccl_unique_id(uint8_t* id128) {
   return PA_OK;
 }
 int pa_merge_create_nccl(pa_agg* member, const uint8_t* id128, uint32_t rank, uint32_t world, pa_merge** out) {
+  if (member && refuse_registered(member)) return PA_EINVAL;
   if (!member || !id128 || !out || world == 0 || world > (uint32_t)kMaxWorld || rank >= world) return PA_EINVAL;
   NcclApi* n = nccl_api();
   if (!n) return PA_EIO;
@@ -1667,6 +1678,7 @@ int pa_merge_create_nccl(pa_agg* member, const uint8_t* id128, uint32_t rank, ui
   return PA_OK;
 }
 int pa_merge_create_host(pa_agg* member, const pa_merge_host_transport* t, uint32_t rank, uint32_t world, pa_merge** out) {
+  if (member && refuse_registered(member)) return PA_EINVAL;
   if (!member || !t || !out || world == 0 || world > (uint32_t)kMaxWorld || rank >= world || !t->allgather || !t->allgatherv || !t->alltoallv || !t->allreduce_min_u32)
     return PA_EINVAL;
   pa_merge* g = new pa_merge();
@@ -1682,6 +1694,7 @@ int pa_merge_create_host(pa_agg* member, const pa_merge_host_transport* t, uint3
   return PA_OK;
 }
 int pa_merge_create_shm(pa_agg* member, const char* name, uint32_t rank, uint32_t world, uint64_t mailbox_bytes, pa_merge** out) {
+  if (member && refuse_registered(member)) return PA_EINVAL;
   if (!member || !name || name[0] != '/' || !out || world == 0 || world > (uint32_t)kMaxWorld || rank >= world) return PA_EINVAL;
   if (mailbox_bytes == 0) mailbox_bytes = 64ull << 20;
   mailbox_bytes = (mailbox_bytes + 4095) & ~4095ull;

@@ -12,7 +12,8 @@ namespace parca {
 namespace {
 struct AggSink final : Sink {
   pa_agg* a;
-  explicit AggSink(pa_agg* agg) : a(agg) {}
+  uint32_t hash_mode;
+  AggSink(pa_agg* agg, uint32_t mode) : a(agg), hash_mode(mode) {}
   uint32_t RegisterString(const std::string& s) override {
     uint32_t off[2] = {0, (uint32_t)s.size()}, id = PA_NO_STRING;
     if (pa_agg_register_strings(a, (const uint8_t*)s.data(), off, 1, &id) != PA_OK) return PA_NO_STRING;
@@ -40,9 +41,15 @@ struct AggSink final : Sink {
     pend_f.clear();
     return rc;
   }
+  uint64_t RegisterStack(const TraceHash& h, const uint64_t* ids, uint32_t n) override {
+    const uint64_t hash[2] = {h.hi, h.lo}, off[2] = {0, n};
+    uint64_t id = ~0ull;
+    if (pa_agg_register_stacks(a, hash_mode == PA_HASH_PROVIDED ? hash : nullptr, ids, off, 1, &id) != PA_OK) return ~0ull;
+    return id;
+  }
   int Submit(const pa_sample_hdr& hdr, const uint64_t* frame_ids) override {
     pend_h.push_back(hdr);
-    pend_f.insert(pend_f.end(), frame_ids, frame_ids + hdr.nframes);
+    if (frame_ids) pend_f.insert(pend_f.end(), frame_ids, frame_ids + hdr.nframes);  // (registered stacks: the row names its stack)
     return pend_h.size() >= kBatch ? push() : PA_OK;
   }
   int Publish() override { return push(); }
@@ -52,7 +59,7 @@ struct AggSink final : Sink {
   int Stacktraces(const uint8_t* ids, uint64_t n, pa_agg_result* out) override { return pa_agg_stacktraces(a, ids, n, out); }
 };
 }  // namespace
-Sink* NewAggSink(pa_agg* agg) { return new AggSink(agg); }
+Sink* NewAggSink(pa_agg* agg, uint32_t hash_mode) { return new AggSink(agg, hash_mode); }
 
 // ---- maybeFixTruncation (reporter/parca_reporter.go:190-216) -------------------------------------
 bool MaybeFixTruncation(std::string* s, size_t maxLen) {
@@ -108,6 +115,8 @@ void ParcaReporter::ReportExecutable(const ExecutableMetadata& md) {
     unknown_by_file_.erase(it);
     trace_cache_.clear();  // cached id lists may contain the forgotten ids
     trace_ids_.clear();
+    stack_cache_.clear();  // and so may registered stacks: their next sighting registers them again
+    zero_hash_stacks_.clear();
   }
 }
 
@@ -219,7 +228,38 @@ int ParcaReporter::writeSampleV2(const Trace* trace, const TraceEventMeta* meta,
   h.cpu = (uint32_t)meta->CPU;
   h.nframes = (uint16_t)nids;
   h.kind = kind;
+  if (cfg_.registeredStacks) {  // `ids` is the stack id: the row carries no frame ids
+    h.frame_off = *ids;
+    return sink_->Submit(h, nullptr);
+  }
   return sink_->Submit(h, ids);
+}
+
+uint64_t ParcaReporter::stackId(const Trace* trace) {
+  const size_t nfr = trace->Frames.size();
+  const bool by_hash = (trace->Hash.hi | trace->Hash.lo) != 0;  // oomprof traces share the zero hash with different frames
+  if (by_hash) {
+    const TraceSlot* tc = stack_cache_.find(trace->Hash);
+    if (tc && tc->n == nfr) return tc->off;
+  }
+  scratch_ids_.clear();
+  scratch_ids_.reserve(nfr);
+  for (auto& f : trace->Frames) scratch_ids_.push_back(frameId(f));
+  std::string key;
+  if (!by_hash) {
+    key.assign((const char*)scratch_ids_.data(), nfr * 8);
+    auto it = zero_hash_stacks_.find(key);
+    if (it != zero_hash_stacks_.end()) return it->second;
+  }
+  const uint64_t id = sink_->RegisterStack(trace->Hash, scratch_ids_.data(), (uint32_t)nfr);
+  if (id == ~0ull) return id;
+  if (by_hash) {
+    if (stack_cache_.size() >= kTraceCacheEntries) stack_cache_.clear();
+    stack_cache_.put(trace->Hash, id, (uint32_t)nfr);
+  } else {
+    zero_hash_stacks_.emplace(std::move(key), id);
+  }
+  return id;
 }
 
 int ParcaReporter::ReportTraceEvent(const Trace* trace, const TraceEventMeta* meta) {
@@ -242,11 +282,15 @@ int ParcaReporter::ReportTraceEvent(const Trace* trace, const TraceEventMeta* me
     }
     labelset = labelsetId(Labels(lb.begin(), lb.end()));
   }
-  // frame ids of this trace: from the per-hash cache when the stack was seen before (one lookup), else per frame
-  const uint64_t* idp = nullptr;
   const size_t nfr = trace->Frames.size();
+  uint64_t stack = 0;
+  if (cfg_.registeredStacks) {  // every row of this trace names its registered stack (writeSampleV2 passes the id, not frames)
+    if (nfr > 65535 || (stack = stackId(trace)) == ~0ull) { droppedBatches++; return 0; }
+  }
+  // frame ids of this trace: from the per-hash cache when the stack was seen before (one lookup), else per frame
+  const uint64_t* idp = cfg_.registeredStacks ? &stack : nullptr;
   const bool cacheable = (trace->Hash.hi | trace->Hash.lo) != 0;  // oomprof traces share the zero hash with different frames
-  if (cacheable) {
+  if (cacheable && !idp) {
     const TraceSlot* tc = trace_cache_.find(trace->Hash);
     if (tc && tc->n == nfr) idp = trace_ids_.data() + tc->off;
   }
@@ -262,7 +306,7 @@ int ParcaReporter::ReportTraceEvent(const Trace* trace, const TraceEventMeta* me
     idp = scratch_ids_.data();
   }
   if (nfr > 65535) { droppedBatches++; return 0; }  // the row format carries a 16-bit depth; such a trace cannot come out of the unwinder
-  const uint64_t* ids = idp;
+  const uint64_t* ids = idp;  // (registered stacks: the stack id)
 
   int rc = 0;
   switch (meta->Origin) {  // reportTraceEventV2 :338-363

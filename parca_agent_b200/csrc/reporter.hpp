@@ -87,6 +87,8 @@ struct Sink {
   virtual uint64_t RegisterFrame(const pa_frame_desc& d) = 0;
   virtual uint32_t RegisterLabelset(const std::vector<pa_label_pair>& pairs) = 0;
   virtual int Submit(const pa_sample_hdr& hdr, const uint64_t* frame_ids) = 0;  // may buffer rows until Publish
+  // Config::registeredStacks: register one stack (its trace hash and frame ids); returns its stack id, ~0 on failure
+  virtual uint64_t RegisterStack(const TraceHash& /*hash*/, const uint64_t* /*ids*/, uint32_t /*n*/) { return ~0ull; }
   virtual int Publish() { return 0; }  // hand buffered rows to the aggregator; called under the reporter's ingest lock
   virtual int Flush(pa_agg_result* out) = 0;
   virtual void Release(pa_agg_result* res) = 0;
@@ -94,7 +96,9 @@ struct Sink {
   virtual int LastStackIds(uint8_t* /*out*/, uint64_t /*n*/) { return PA_EINVAL; }
   virtual int Stacktraces(const uint8_t* /*ids*/, uint64_t /*n*/, pa_agg_result* /*out*/) { return PA_EINVAL; }
 };
-Sink* NewAggSink(pa_agg* agg);  // owns nothing; forwards to the C ABI
+// owns nothing; forwards to the C ABI. hash_mode: the aggregator's (RegisterStack passes the trace hash in PA_HASH_PROVIDED mode
+// only; in PA_HASH_XXH64X2 mode the library computes the stack id)
+Sink* NewAggSink(pa_agg* agg, uint32_t hash_mode = PA_HASH_PROVIDED);
 
 struct Config {
   std::string nodeName;
@@ -109,6 +113,10 @@ struct Config {
   // v1 schema in offline mode (:1262-1349): after every sample record, the stacktrace record of the stacks this log
   // has not seen yet is appended as a second batch. The aggregator behind the sink must be a PA_SCHEMA_V1 one.
   bool offlineV1Stacktraces = false;
+  // registered stacks (PA_CFG_REGISTERED_STACKS aggregator behind the sink): each distinct trace is registered once through
+  // Sink::RegisterStack and its rows carry the stack id in frame_off with no frame ids. Traces are keyed by trace.Hash, the
+  // zero hash (oomprof traces) by the frame-id list.
+  bool registeredStacks = false;
 };
 
 class ParcaReporter {
@@ -191,6 +199,9 @@ class ParcaReporter {
   } trace_cache_;
   std::vector<uint64_t> trace_ids_;
   std::vector<uint64_t> scratch_ids_;
+  // Config::registeredStacks: trace.Hash -> stack id (off = the id, n = the depth), and frame-id list -> stack id for the zero hash
+  TraceCache stack_cache_;
+  std::unordered_map<std::string, uint64_t> zero_hash_stacks_;
   static constexpr size_t kTraceCacheEntries = 1u << 20;
   std::map<FileID, ExecutableMetadata> executables_;          // r.executables (:650-693)
   std::map<FileID, std::vector<std::string>> unknown_by_file_;  // frames interned while their executable was unknown
@@ -207,6 +218,7 @@ class ParcaReporter {
   uint32_t labelsetId(const Labels& l);
   bool labelsForPID(uint32_t pid, PidLabels** out);
   int writeSampleV2(const Trace* trace, const TraceEventMeta* meta, uint32_t labelset, uint8_t kind, int64_t value, const uint64_t* ids, size_t nids);
+  uint64_t stackId(const Trace* trace);  // Config::registeredStacks: the trace's stack id, registered on first sight; ~0 = failed
 };
 
 // maybeFixTruncation (parca_reporter.go:190-216)

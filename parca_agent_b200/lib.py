@@ -16,7 +16,7 @@ _LIB = None
 
 EXPORTS = [
     "pa_agg_create", "pa_agg_destroy", "pa_agg_last_error", "pa_agg_abi_version", "pa_agg_register_strings",
-    "pa_agg_register_frames", "pa_agg_register_labelsets", "pa_agg_acquire", "pa_agg_commit", "pa_agg_submit",
+    "pa_agg_register_frames", "pa_agg_register_labelsets", "pa_agg_register_stacks", "pa_agg_acquire", "pa_agg_commit", "pa_agg_submit",
     "pa_agg_flush", "pa_agg_release", "pa_agg_stage", "pa_agg_process", "pa_agg_collect", "pa_agg_last_kernel_ms",
     "pa_agg_debug_stack_ids", "pa_agg_debug_stack_counts", "pa_agg_debug_pair_counts", "pa_agg_stacktraces", "pa_agg_last_stack_ids", "pa_agg_shard_sizes", "pa_agg_shard_export", "pa_agg_stage_device", "pa_agg_stage_device_parts", "pa_agg_discard", "pa_ipc_compress_lz4", "pa_ipc_free", "pa_fix_truncation", "pa_xxh64",
     "pa_merge_create_local", "pa_merge_nccl_unique_id", "pa_merge_create_nccl", "pa_merge_destroy", "pa_merge_last_error", "pa_merge_process",
@@ -48,6 +48,7 @@ def lib():
         L.pa_agg_register_strings.argtypes = [vp, C.c_char_p, vp, C.c_uint32, u32p]
         L.pa_agg_register_frames.argtypes = [vp, vp, C.c_uint32, u64p]
         L.pa_agg_register_labelsets.argtypes = [vp, vp, vp, C.c_uint32, u32p]
+        L.pa_agg_register_stacks.argtypes = [vp, vp, vp, vp, C.c_uint32, u64p]
         L.pa_agg_acquire.argtypes = [vp, C.c_uint64, C.c_uint64, C.POINTER(vp), C.POINTER(vp), u64p]
         L.pa_agg_commit.argtypes = [vp, C.c_uint64]
         L.pa_agg_submit.argtypes = [vp, vp, vp, C.c_uint64]
@@ -135,6 +136,7 @@ class Aggregator:
         self.h = h
         self.max_samples = max_samples
         self.id_dtype = np.uint32 if frame_id_bytes == 4 else np.uint64  # what the ring holds per frame id
+        self.registered = bool(flags & abi.PA_CFG_REGISTERED_STACKS)
 
     def _ck(self, rc):
         if rc != 0:
@@ -170,6 +172,19 @@ class Aggregator:
         self._ck(lib().pa_agg_register_labelsets(self.h, pairs.ctypes.data, offs.ctypes.data, len(labelsets), C.byref(first)))
         return first.value
 
+    def register_stacks(self, frames, offsets, hashes=None):
+        """PA_CFG_REGISTERED_STACKS: stack i = frames[offsets[i]:offsets[i+1]]; hashes (n, 2) [hash_hi, hash_lo] in
+        PA_HASH_PROVIDED mode, None in PA_HASH_XXH64X2 mode. Returns the id of the first stack."""
+        frames = np.ascontiguousarray(frames, dtype=self.id_dtype)
+        offsets = np.ascontiguousarray(offsets, dtype=np.uint64)
+        n = len(offsets) - 1
+        if hashes is not None:
+            hashes = np.ascontiguousarray(hashes, dtype=np.uint64).reshape(-1)
+        first = C.c_uint64()
+        self._ck(lib().pa_agg_register_stacks(self.h, None if hashes is None else hashes.ctypes.data, frames.ctypes.data if len(frames) else None,
+                                              offsets.ctypes.data, n, C.byref(first)))
+        return first.value
+
     # ---- ingest
     def submit(self, hdrs, frame_ids):
         hdrs = np.ascontiguousarray(hdrs, dtype=abi.HDR_DTYPE)
@@ -183,6 +198,8 @@ class Aggregator:
         self._ck(lib().pa_agg_acquire(self.h, n_rows, n_frames, C.byref(ph), C.byref(pf), C.byref(base)))
         hv = np.ctypeslib.as_array(C.cast(ph, C.POINTER(C.c_uint8)), shape=(max(n_rows, 1) * 64,))[:n_rows * 64].view(abi.HDR_DTYPE)
         ctype = C.c_uint32 if self.id_dtype == np.uint32 else C.c_uint64
+        if not pf.value:  # registered stacks: the ring holds no frame ids
+            return hv, np.zeros(0, self.id_dtype), base.value
         fv = np.ctypeslib.as_array(C.cast(pf, C.POINTER(ctype)), shape=(max(n_frames, 1),))[:n_frames]
         return hv, fv, base.value
 
@@ -380,21 +397,90 @@ class _HeadlessResult(Result):
         self.ipc_len = n
 
 
-def from_workload(w, device=0, max_samples=None, max_frames=None, chunk_samples=0, **kw):
-    """Aggregator with the workload's dictionaries registered (string id 0 == "" is implicit)."""
+class StackForm:
+    """A workload's rows in registered-stacks form: stack i = frames[offsets[i]:offsets[i+1]] with the stack id
+    hashes[i] = (hash_hi, hash_lo) its rows carry, and stack_of_row[r] = the stack row r names (its frame_off)."""
+
+    def __init__(self, hashes, frames, offsets, stack_of_row):
+        self.hashes, self.frames, self.offsets, self.stack_of_row = hashes, frames, offsets, stack_of_row
+
+
+def stack_form(w):
+    """Workloads with a stack table register the table, with the id of each stack taken from the rows that name it (stacks no
+    row names get id 0); the others (explicit frame streams) are deduplicated on (hash_hi, hash_lo, frame ids)."""
+    if w._frame_ids is None:
+        t = np.ascontiguousarray(w.stack_table, dtype=np.uint64)
+        hashes = np.zeros((t.shape[0], 2), dtype=np.uint64)
+        hashes[w.stack_choice, 0] = w.hdrs["hash_hi"]
+        hashes[w.stack_choice, 1] = w.hdrs["hash_lo"]
+        offsets = np.arange(t.shape[0] + 1, dtype=np.uint64) * np.uint64(t.shape[1])
+        return StackForm(hashes, t.reshape(-1), offsets, np.asarray(w.stack_choice, dtype=np.uint64))
+    ids = w.frame_ids
+    index, hashes, parts = {}, [], []
+    of_row = np.zeros(w.n, dtype=np.uint64)
+    for r, (hi, lo, off, nf) in enumerate(zip(w.hdrs["hash_hi"].tolist(), w.hdrs["hash_lo"].tolist(), w.hdrs["frame_off"].tolist(), w.hdrs["nframes"].tolist())):
+        fr = ids[off:off + nf]
+        key = (hi, lo, fr.tobytes())
+        s = index.get(key)
+        if s is None:
+            s = index[key] = len(parts)
+            hashes.append((hi, lo))
+            parts.append(fr)
+        of_row[r] = s
+    offsets = np.zeros(len(parts) + 1, dtype=np.uint64)
+    offsets[1:] = np.cumsum([len(p) for p in parts], dtype=np.uint64)
+    frames = np.concatenate(parts).astype(np.uint64) if parts else np.zeros(0, np.uint64)
+    return StackForm(np.asarray(hashes, dtype=np.uint64).reshape(-1, 2), frames, offsets, of_row)
+
+
+def expand_stack_form(hdrs, sf):
+    """The ring form of rows in registered-stacks form: (headers with hash_hi / hash_lo / nframes / frame_off of their stack,
+    concatenated frame ids) — what an aggregator without PA_CFG_REGISTERED_STACKS ingests for the same samples."""
+    hd = np.array(hdrs, dtype=abi.HDR_DTYPE, copy=True)
+    s = np.asarray(sf.stack_of_row, dtype=np.int64)
+    start, end = sf.offsets[:-1].astype(np.int64), sf.offsets[1:].astype(np.int64)
+    nf = (end - start)[s]
+    hd["hash_hi"], hd["hash_lo"] = sf.hashes[s, 0], sf.hashes[s, 1]
+    hd["nframes"] = nf
+    off = np.zeros(len(s), dtype=np.int64)
+    if len(s):
+        off[1:] = np.cumsum(nf)[:-1]
+    hd["frame_off"] = off.astype(np.uint64)
+    total = int(nf.sum())
+    idx = np.repeat(start[s], nf) + (np.arange(total, dtype=np.int64) - np.repeat(off, nf))
+    return hd, np.asarray(sf.frames, dtype=np.uint64)[idx]
+
+
+def from_workload(w, device=0, max_samples=None, max_frames=None, chunk_samples=0, registered_stacks=False, flags=0, **kw):
+    """Aggregator with the workload's dictionaries registered (string id 0 == "" is implicit). registered_stacks: a
+    PA_CFG_REGISTERED_STACKS aggregator with the workload's stacks registered too (stack_form); max_frames then defaults to
+    the registered frames."""
+    sf = stack_form(w) if registered_stacks else None
     n = max(1, w.n if max_samples is None else max_samples)
-    nf = max(1, w.n_frame_ids if max_frames is None else max_frames)
+    nf = max(1, (len(sf.frames) if sf else w.n_frame_ids) if max_frames is None else max_frames)
     a = Aggregator(device=device, hash_mode=w.hash_mode, label_flags=w.label_flags, samples_per_second=w.samples_per_second,
-                   external_labels=w.external_labels, max_samples=n, max_frames=nf, chunk_samples=chunk_samples, schema=getattr(w, "schema", 0), **kw)
+                   external_labels=w.external_labels, max_samples=n, max_frames=nf, chunk_samples=chunk_samples, schema=getattr(w, "schema", 0),
+                   flags=flags | (abi.PA_CFG_REGISTERED_STACKS if registered_stacks else 0), **kw)
     first = a.register_strings(w.strings[1:])
     assert first == 1, first
     a.register_frames(w.frames)
     a.register_labelsets(w.labelsets)
+    if sf is not None:
+        a.stack_form = sf
+        a.register_stacks(sf.frames, sf.offsets, sf.hashes if w.hash_mode == abi.PA_HASH_PROVIDED else None)
     return a
 
 
-def load(a, w):
-    """Write the workload's rows straight into the pinned ring (no intermediate copy of the frame stream)."""
+def load(a, w, stack_of_row=None):
+    """Write the workload's rows straight into the pinned ring (no intermediate copy of the frame stream). On a registered-stacks
+    aggregator the rows name registered stacks (stack_of_row, by default those from_workload(w, registered_stacks=True)
+    registered) and the ring gets no frames."""
+    if a.registered:
+        hv, _, _ = a.acquire(w.n, 0)
+        hv[:] = w.hdrs
+        hv["frame_off"] = a.stack_form.stack_of_row if stack_of_row is None else stack_of_row
+        a.commit(w.n)
+        return
     hv, fv, base = a.acquire(w.n, w.n_frame_ids)
     hv[:] = w.hdrs
     if base:

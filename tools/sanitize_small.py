@@ -8,7 +8,9 @@ narrow ring, and a v1 batch with its stacktrace record, each checked against the
 merge_lz4_gpu: a small in-process merge group of PA_IPC_LZ4_FRAME_GPU members whose shard cuts put blocks across part borders
 (heads exchange, crossing blocks, an empty shard), checked against one such aggregator on the concatenated rows.
 merge_v1: in-process groups of PA_SCHEMA_V1 members over several intervals against a small store (evictions, compaction, an
-over-full batch, stacktrace requests), plain and PA_IPC_LZ4_FRAME_GPU, checked against one v1 aggregator and the oracle."""
+over-full batch, stacktrace requests), plain and PA_IPC_LZ4_FRAME_GPU, checked against one v1 aggregator and the oracle.
+registered: PA_CFG_REGISTERED_STACKS aggregators (both hash modes, the narrow ring, small chunks, v1) against the oracle, and a
+row naming an unregistered stack id followed by a clean flush."""
 import os
 import sys
 
@@ -74,8 +76,37 @@ def merge_v1():
     print("sanitize_small merge_v1 ok")
 
 
+def registered():
+    """PA_CFG_REGISTERED_STACKS: both hash modes, narrow ids, small chunks, v1, a row naming an unregistered stack"""
+    for mode in (abi.PA_HASH_PROVIDED, abi.PA_HASH_XXH64X2):
+        w = synth.edge_workload(seed=3, n=3000, hash_mode=mode, external=False)
+        for kw in ({}, {"frame_id_bytes": 4, "chunk_samples": 700}):
+            got, _ = lib.run(w, registered_stacks=True, **kw)
+            assert got == oracle_py.run(w)[0]
+        w.schema = abi.PA_SCHEMA_V1
+        got, _ = lib.run(w, registered_stacks=True)
+        assert got == oracle_py.run(w)[0]
+    w = synth.ragged(n=3000, u=300, p=1024)
+    a = lib.from_workload(w, registered_stacks=True)
+    hv, _, _ = a.acquire(2, 0)
+    hv[:] = w.hdrs[:2]
+    hv["frame_off"] = [0, 1 << 40]
+    a.commit(2)
+    try:
+        a.flush()
+        raise AssertionError("an unregistered stack id must fail the flush")
+    except lib.PaError:
+        pass
+    lib.load(a, w)
+    assert a.flush().ipc_bytes() == oracle_py.run(w)[0]
+    a.close()
+    print("sanitize_small registered ok")
+
+
 def main():
     oracle_py.build()
+    if sys.argv[1:] == ["registered"]:
+        return registered()
     if sys.argv[1:] == ["lz4_gpu"]:
         return lz4_gpu()
     if sys.argv[1:] == ["merge_lz4_gpu"]:
