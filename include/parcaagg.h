@@ -90,7 +90,16 @@ enum {
                                     and hands out *frames = NULL; pa_agg_submit ignores `frames` and keeps the caller's frame_off. A row
                                     whose stack id is not registered fails the flush with PA_EINVAL (the next flush works).
                                     max_frames (0 = max_samples * 64) bounds the registered frames instead of the ring.
-                                    Not supported yet (PA_EINVAL): pa_merge_create_*, pa_agg_shard_export, pa_agg_stage_device(_parts) */
+                                    Not supported (PA_EINVAL): pa_agg_shard_export, pa_agg_stage_device(_parts); and pa_merge_create_*
+                                    unless PA_CFG_GROUP_STACKS is set too */
+#define PA_CFG_GROUP_STACKS 0x4u /* with PA_CFG_REGISTERED_STACKS only (pa_agg_create fails with PA_EINVAL otherwise): the stack ids
+                                    are group-wide, so the aggregator may be a member of a merge group. Every member of such a group
+                                    registers the same stacks in the same order (like strings, frames and labelsets), so a row's
+                                    frame_off names the same stack on every shard; pa_merge_process checks the count, the arena length
+                                    and a digest of (id, depth, frame ids) of the registered stacks and fails with PA_EINVAL on every
+                                    rank when they differ. A group cannot mix such members with ring members (pa_merge_create_local
+                                    refuses it, multi-process groups fail pa_merge_process on every rank). On its own the aggregator
+                                    behaves exactly like a PA_CFG_REGISTERED_STACKS one */
 
 #define PA_NO_STRING 0xFFFFFFFFu /* "no value"; string id 0 is always the empty string "" */
 
@@ -328,7 +337,9 @@ int pa_agg_stage_device_parts(pa_agg* a, const pa_device_part* parts, uint32_t n
  * the "store_evictions" / "store_compactions" counters. Every member holds a full copy of the group's known-stacks store and
  * pa_merge_process applies the merged batch's accesses to each copy (it exchanges the global last row of every merged stack and
  * the frames of the stacks the store lacks; pa_agg_last_kernel_ms(member, "store_frames", ...) reports, in *launches, the frame
- * ids the member sent in the last pa_merge_process). An error any member's store update finds (e.g. an unregistered frame id,
+ * ids the member sent in the last pa_merge_process). PA_CFG_GROUP_STACKS groups send one 8-byte offset into the registered frame
+ * arena per stack instead of its frames (every member holds the same arena): "store_refs" reports those offsets the same way,
+ * and "store_frames" is 0. An error any member's store update finds (e.g. an unregistered frame id,
  * seen only by the shard that sends that stack's frames) fails pa_merge_process on every rank. After a merged interval pa_agg_last_stack_ids on any member returns the merged dictionary, and a member
  * flushed on its own continues from the group's store. A group that mixes schemas, or v1 members with different store sizes, is
  * refused like a mixed LZ4 group (pa_merge_create_local at once, with the reason in every member's pa_agg_last_error;

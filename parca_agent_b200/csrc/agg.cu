@@ -108,6 +108,7 @@ struct Pass {
   uint32_t n_cstr = 0, n_frames = 0, n_funcs = 0, n_sids = 0, n_labelsets = 0;
   uint32_t n_stacks = 0;          // registered stacks (PA_CFG_REGISTERED_STACKS)
   uint64_t n_stack_frames = 0;    // and the frame ids of their arena
+  uint64_t stack_digest = 0;      // PA_CFG_GROUP_STACKS: digest of those stacks (merge groups check it is the same on every member)
   uint64_t N = 0, NT = 0, row_base = 0;
   uint32_t world = 1, rank = 0, ncols = 0, nlab = 0;
   bool v1 = false, provided = false, merged = false;  // provided: the stack ids arrive with the rows (or their registered stacks)
@@ -185,6 +186,8 @@ struct pa_agg {
   DBuf d_lsmat, d_kindtab, d_cols, d_jobs;
   // PA_CFG_REGISTERED_STACKS: the registered stacks and their frame arena (ids at the ring's width, idb / 4 words each)
   bool registered = false;
+  bool group_stacks = false;  // PA_CFG_GROUP_STACKS: the stack ids are group-wide (merge groups)
+  uint64_t reg_digest = 0;    // PA_CFG_GROUP_STACKS: running digest of every registered stack's (id, depth, frame ids)
   std::vector<RegStack> reg_stacks;
   std::vector<uint32_t> reg_arena;
   Mirror<RegStack> m_stacks;
@@ -200,6 +203,7 @@ struct pa_agg {
   uint32_t* h_select = nullptr;              // pinned: 256-bin histogram of a select pass, then a StoreCtl read-back
   uint64_t store_compactions = 0, store_evictions = 0;
   uint64_t store_frames_sent = 0;            // v1 merge groups: frame ids this member sent in the last store exchange
+  uint64_t store_refs_sent = 0;              // v1 PA_CFG_GROUP_STACKS merge groups: the arena offsets it sent instead
   uint32_t cid_unknown = 0, cid_missing = 0;  // "unknown" (libpf.UnknownFrame.String()) and "missing stacktrace" (:1561, :1568)
 
   // ---- ring (pinned host), double buffered
@@ -386,6 +390,7 @@ const char* pa_agg_last_error(const pa_agg* a) { return a ? a->err.c_str() : "nu
 int pa_agg_create(const pa_agg_config* cfg, pa_agg** out) {
   if (!cfg || !out || cfg->abi_version != PA_ABI_VERSION || cfg->samples_per_second == 0 || cfg->max_samples == 0 || cfg->hash_mode > 1 || cfg->schema > 1 || cfg->ipc_compression > PA_IPC_LZ4_FRAME_GPU ||
       (cfg->frame_id_bytes != 0 && cfg->frame_id_bytes != 4 && cfg->frame_id_bytes != 8)) return PA_EINVAL;
+  if ((cfg->flags & PA_CFG_GROUP_STACKS) && !(cfg->flags & PA_CFG_REGISTERED_STACKS)) return PA_EINVAL;
   if (cfg->max_samples > 0x7FFFFFFFull) return PA_ERANGE;  // run ends / ListView offsets are int32
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || cfg->device < 0 || cfg->device >= ndev) return PA_ENODEV;
@@ -397,6 +402,7 @@ int pa_agg_create(const pa_agg_config* cfg, pa_agg** out) {
   a->idb = cfg->frame_id_bytes == 4 ? 4u : 8u;
   a->single_ring = (cfg->flags & PA_CFG_SINGLE_RING) != 0;
   a->registered = (cfg->flags & PA_CFG_REGISTERED_STACKS) != 0;
+  a->group_stacks = (cfg->flags & PA_CFG_GROUP_STACKS) != 0;
   auto bail = [&](int code) { pa_agg_destroy(a); return code; };
   if (cudaSetDevice(a->device) != cudaSuccess) return bail(PA_ENODEV);
   cudaDeviceProp prop;
@@ -627,6 +633,12 @@ int pa_agg_register_stacks(pa_agg* a, const uint64_t* hashes, const uint64_t* fr
       s.hash_hi = pa_xxh64(wide.data(), d * 8, 0);
       s.hash_lo = pa_xxh64(wide.data(), d * 8, PA_XXH_SEED_LO);
     }
+    if (a->group_stacks) {  // the registry's digest: XXH64 of (hash_hi, hash_lo, depth, frame ids as uint64), seeded with the digest so far
+      wide.resize(d + 3);
+      wide[0] = s.hash_hi; wide[1] = s.hash_lo; wide[2] = d;
+      for (uint64_t j = 0; j < d; j++) wide[3 + j] = a->idb == 4 ? (uint64_t)f32[offsets[i] + j] : frames[offsets[i] + j];
+      a->reg_digest = pa_xxh64(wide.data(), (d + 3) * 8, a->reg_digest);
+    }
     a->reg_stacks.push_back(s);
   }
   return PA_OK;
@@ -800,6 +812,7 @@ static int upload_tables(pa_agg* a) {
     CK(a->m_stacks.sync(a->reg_stacks, s)); CK(a->m_arena.sync(a->reg_arena, s));
     a->src_frames = (const unsigned long long*)a->m_arena.ptr();  // (a regrown mirror moves: set on every upload)
     a->P.n_stacks = (uint32_t)a->reg_stacks.size(); a->P.n_stack_frames = a->reg_arena.size() / (a->idb / 4);
+    a->P.stack_digest = a->reg_digest;
   }
   // what the device mirrors now hold: the pass uses these counts only (registration may continue concurrently)
   a->P.n_cstr = a->sp.count(); a->P.n_frames = a->ft.count(); a->P.n_funcs = a->ft.n_funcs();
@@ -2715,6 +2728,13 @@ int pa_agg_last_kernel_ms(const pa_agg* a, const char* name, double* ms, uint32_
   if (!strcmp(name, "store_frames")) {
     if (ms) *ms = 0;
     if (launches) *launches = (uint32_t)std::min<uint64_t>(a->store_frames_sent, 0xFFFFFFFFu);
+    return PA_OK;
+  }
+  // PA_SCHEMA_V1 merge groups of PA_CFG_GROUP_STACKS members (ms is 0): stack references (8-byte arena offsets) this member sent
+  // instead of frame ids in the last store exchange
+  if (!strcmp(name, "store_refs")) {
+    if (ms) *ms = 0;
+    if (launches) *launches = (uint32_t)std::min<uint64_t>(a->store_refs_sent, 0xFFFFFFFFu);
     return PA_OK;
   }
   return PA_EINVAL;

@@ -2351,6 +2351,9 @@ struct StoreInsertArgs {
   const uint32_t* g_last_inv;        // [U] 0xFFFFFFFF - global last row
   const uint32_t* g_frames;          // frames of the stacks the store lacks, gathered from the shards that hold their first occurrence
   const unsigned long long* g_foff;  // [U + 1] where each ordinal's frames start in g_frames (an ordinal without frames there: equal neighbours)
+  // k_store_insert<true, true> (PA_CFG_GROUP_STACKS): g_foff indexes g_refs instead, one entry per stack; the frames are read from
+  // this member's own registered arena (`frames`), which is the same on every member
+  const unsigned long long* g_refs;  // arena offset of each needed stack's frames, from its global first occurrence
 };
 // last occurrence of every stack of the batch (the LRU's access time of its entry)
 __global__ void __launch_bounds__(kThreads) k_last_rows(uint32_t n_rows, const uint32_t* slot_of_row, uint32_t* last_row) {
@@ -2393,7 +2396,8 @@ __global__ void __launch_bounds__(kThreads) k_store_kill(unsigned long long* sta
 }
 // one warp per unique stack of the batch (unique within the launch, so a key is claimed by at most one warp).
 // MERGED: one replica of a merge group's store; u is the merged ordinal, frames come from the gathered buffer.
-template <bool MERGED>
+// REFS (with MERGED): frames come from the member's registered arena, at the gathered offset (g_refs).
+template <bool MERGED, bool REFS = false>
 __global__ void __launch_bounds__(kThreads) k_store_insert(StoreInsertArgs a) {
   const unsigned full = 0xFFFFFFFFu;
   uint32_t nu = a.ctr->n_unique;
@@ -2456,7 +2460,19 @@ __global__ void __launch_bounds__(kThreads) k_store_insert(StoreInsertArgs a) {
     fresh = __shfl_sync(full, fresh, 0);
     if (!fresh) continue;
     off = __shfl_sync(full, off, 0);
-    if constexpr (MERGED) {  // the frames were checked where they were packed (k_store_pack)
+    if constexpr (MERGED && REFS) {
+      const unsigned long long k = a.g_foff[u];
+      if (a.g_foff[u + 1] - k != (size ? 1u : 0u)) {  // not in the gathered set: a logic error, reported instead of storing garbage
+        if (lane == 0) atomicOr(&a.ctr_w->err, ERR_MERGE_LOOKUP);
+        continue;
+      }
+      const unsigned long long base = size ? a.g_refs[k] : 0ull;
+      for (uint32_t j = lane; j < size; j += 32) {
+        unsigned long long fid = frame_at(a.frames, base + j, a.narrow);
+        if (fid >= a.n_frames_registered) { atomicOr(&a.ctr_w->err, ERR_BAD_FRAME_ID); fid = 0; }
+        a.arena[off + j] = (uint32_t)fid;
+      }
+    } else if constexpr (MERGED) {  // the frames were checked where they were packed (k_store_pack)
       const unsigned long long base = a.g_foff[u];
       if (a.g_foff[u + 1] - base != size) {  // not in the gathered set: a logic error, reported instead of storing garbage
         if (lane == 0) atomicOr(&a.ctr_w->err, ERR_MERGE_LOOKUP);
@@ -3021,6 +3037,27 @@ __global__ void __launch_bounds__(kThreads) k_store_pack(const MergeCtl* mc, con
       out[dst + j] = (uint32_t)fid;
     }
   }
+}
+// PA_CFG_GROUP_STACKS groups: every member holds the same registered arena, so a stack the store lacks crosses as one reference
+// instead of its frames — the arena offset of its global first occurrence (the row's frame_off after k_header<true>), which
+// keeps that occurrence's frames when two registered stacks share a provided id
+struct StoreRefsF {  // where each merged stack's reference goes in the gathered buffer: exclusive scan of (k_store_need != 0)
+  typedef unsigned long long T;
+  const Counters* ctr;
+  const uint32_t* need;
+  unsigned long long* ridx;
+  __device__ uint32_t n() const { return ctr->n_unique; }
+  __device__ unsigned long long value(uint32_t u) const { return need[u] ? 1ull : 0ull; }
+  __device__ void emit(uint32_t u, unsigned long long ex, unsigned long long) const { ridx[u] = ex; }
+  __device__ void total(int, unsigned long long t) const { ridx[ctr->n_unique] = t; }
+};
+// this shard's block: the references of its won stacks that k_store_need selected
+__global__ void __launch_bounds__(kThreads) k_store_pack_refs(const MergeCtl* mc, const uint32_t* g_row, uint32_t row_base, const uint32_t* need,
+                                                              const unsigned long long* ridx, const unsigned long long* frame_off, unsigned long long* out) {
+  const uint32_t o0 = mc->ord0, o1 = mc->ord1;
+  const unsigned long long base0 = ridx[o0];
+  for (uint32_t u = o0 + blockIdx.x * kThreads + threadIdx.x; u < o1; u += gridDim.x * kThreads)
+    if (need[u]) out[ridx[u] - base0] = frame_off[g_row[u] - row_base];
 }
 
 // ---------------------------------------------------------------------------------------------

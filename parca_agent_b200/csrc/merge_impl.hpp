@@ -12,6 +12,7 @@
 //   all-gather   thread-id lists, per-column run edges (count, first / last key)                      T x 8 B + cols x 40 B
 //   v1 groups (replicated known-stacks store): all-reduce(min) of each merged stack's inverted last row  U x 4 B
 //                and all-gather-v of the frames of the stacks the store lacks                          4 B per frame (0 in steady state)
+//                (PA_CFG_GROUP_STACKS members: of one arena offset per such stack instead)             8 B per stack
 // Invariants reproduced: first-occurrence order of every dictionary (arrow_v2.go:191, :302; parca_reporter.go:425),
 // run merging across shard borders (arrow.go:97-131).
 //
@@ -150,6 +151,8 @@ struct pa_merge {
   uint64_t registered_len = 0;
   // ---- PA_IPC_LZ4_FRAME_GPU groups (every member in that mode): LZ4_FRAME bodies on the whole buffers' 64 KiB block grid
   bool lz4 = false;
+  // ---- PA_CFG_GROUP_STACKS groups (every member in that mode): rows name stacks of identical registries, no ring frames
+  bool group_stacks = false;
   struct Lz4Share {                             // one local member's blocks, from pa_merge_plan to pa_merge_collect
     Lz4Table t;
     Lz4Dev d;
@@ -185,6 +188,12 @@ namespace pa {
 static bool lz4_gpu_member(const pa_agg* m) { return m->cfg.ipc_compression == PA_IPC_LZ4_FRAME_GPU; }
 static const char kLz4Mixed[] = "a merge group builds LZ4_FRAME records only when every member uses PA_IPC_LZ4_FRAME_GPU, and plain ones when none does: "
                                 "this group mixes PA_IPC_LZ4_FRAME_GPU members with other members";
+// Registered stacks join a group only with group-wide ids (PA_CFG_GROUP_STACKS), and only groups where every member has them.
+static bool group_stacks_member(const pa_agg* m) { return m->group_stacks; }
+static const char kStacksMixed[] = "a merge group of PA_CFG_GROUP_STACKS members takes no other members: this group mixes PA_CFG_GROUP_STACKS members "
+                                   "with ring members or with plain PA_CFG_REGISTERED_STACKS members";
+static const char kStacksMismatch[] = "the members of a PA_CFG_GROUP_STACKS merge group must register identical stacks in the same order: "
+                                      "their number of stacks, frame arena length or stack digest differ";
 // Every member of a group uses the same schema; v1 members also need the same store size, since each holds a full copy of the
 // group's store (refused like a mixed LZ4 mode).
 static const char kSchemaMixed[] = "a merge group builds one record schema: this group mixes PA_SCHEMA_V1 and PA_SCHEMA_V2 members";
@@ -807,11 +816,14 @@ static int merge_process_once(pa_merge* g, bool* retry) {
 // over U words), and the frames of the stacks the store lacks, each sent by the shard that holds its global first occurrence
 // (all-gather-v; near zero in steady state). Every decision below depends only on replicated state, so every rank takes it.
 
-// the frames the insert may need (k_store_need on the store as it is now), gathered into every member's v1_frames
+// the frames the insert may need (k_store_need on the store as it is now), gathered into every member's v1_frames; in
+// PA_CFG_GROUP_STACKS groups one arena offset per such stack instead (v1_foff then indexes references, not frames)
 static int store_frames_exchange(pa_merge* g, uint32_t min_last_p1) {
   const size_t L = g->members.size();
   const uint32_t W = g->world;
   const uint64_t U = g->members[0]->h_ctr.n_unique;
+  const bool refs = g->group_stacks;
+  const uint64_t unit = refs ? 8 : 4;
   std::vector<std::vector<uint64_t>> bounds(L, std::vector<uint64_t>(W + 1));
   RankRows rr{};
   for (uint32_t r = 0; r <= W; r++) rr.base[r] = (uint32_t)g->row_base[r];
@@ -827,7 +839,8 @@ static int store_frames_exchange(pa_merge* g, uint32_t min_last_p1) {
     k_store_need<<<small_grid(a, U), kThreads, 0, s>>>(ctr, mb.gtab.as<StackSlot>(), mb.g_uniq_slot.as<uint32_t>(), mb.v1_last.as<uint32_t>(), min_last_p1,
                                                        a->d_store.as<StoreSlot>(), (uint32_t)(a->store_slots - 1), a->d_store_stamp.as<unsigned long long>(),
                                                        mb.v1_need.as<uint32_t>());
-    launch_scan(a, StoreFramesF{ctr, mb.v1_need.as<uint32_t>(), mb.v1_foff.as<unsigned long long>()}, 1, a->tm[T_RANK], small_grid(a, U), s, a->d_partial);
+    if (refs) launch_scan(a, StoreRefsF{ctr, mb.v1_need.as<uint32_t>(), mb.v1_foff.as<unsigned long long>()}, 1, a->tm[T_RANK], small_grid(a, U), s, a->d_partial);
+    else launch_scan(a, StoreFramesF{ctr, mb.v1_need.as<uint32_t>(), mb.v1_foff.as<unsigned long long>()}, 1, a->tm[T_RANK], small_grid(a, U), s, a->d_partial);
     k_rank_bounds<<<1, kMaxWorld + 32, 0, s>>>(ctr, mb.g_uniq_row.as<uint32_t>(), mb.v1_foff.as<unsigned long long>(), rr, W, mb.v1_bounds.as<unsigned long long>());
     MCK(cudaMemcpyAsync(bounds[i].data(), mb.v1_bounds.p, (W + 1) * 8, cudaMemcpyDeviceToHost, s));
   }
@@ -835,7 +848,7 @@ static int store_frames_exchange(pa_merge* g, uint32_t min_last_p1) {
   if (rc) return rc;
   const std::vector<uint64_t>& b = bounds[0];  // identical on every member
   std::vector<uint64_t> count(W), displ(W);
-  for (uint32_t r = 0; r < W; r++) { displ[r] = b[r] * 4; count[r] = (b[r + 1] - b[r]) * 4; }
+  for (uint32_t r = 0; r < W; r++) { displ[r] = b[r] * unit; count[r] = (b[r + 1] - b[r]) * unit; }
   std::vector<const void*> src(L);
   std::vector<void*> dst(L);
   for (size_t i = 0; i < L; i++) {
@@ -844,7 +857,15 @@ static int store_frames_exchange(pa_merge* g, uint32_t min_last_p1) {
     MergeBufs& mb = g->mb[i];
     const uint32_t me = g->ranks[i];
     MCK(mb.v1_send.ensure(std::max<uint64_t>(count[me], 256)));
-    MCK(mb.v1_frames.ensure(std::max<uint64_t>(b[W] * 4, 256)));
+    MCK(mb.v1_frames.ensure(std::max<uint64_t>(b[W] * unit, 256)));
+    if (refs) {
+      k_store_pack_refs<<<small_grid(a, U), kThreads, 0, a->s_comp>>>((const MergeCtl*)(mb.ctl.as<uint32_t>() + CTL_MERGE), mb.g_uniq_row.as<uint32_t>(),
+                                                                      (uint32_t)g->row_base[me], mb.v1_need.as<uint32_t>(), mb.v1_foff.as<unsigned long long>(),
+                                                                      a->d_foff.as<unsigned long long>(), mb.v1_send.as<unsigned long long>());
+      a->store_refs_sent += count[me] / 8;
+      src[i] = mb.v1_send.p; dst[i] = mb.v1_frames.p;
+      continue;
+    }
     k_store_pack<<<a->G, kThreads, 0, a->s_comp>>>((const MergeCtl*)(mb.ctl.as<uint32_t>() + CTL_MERGE), mb.g_uniq_row.as<uint32_t>(), (uint32_t)g->row_base[me],
                                                    mb.v1_need.as<uint32_t>(), mb.v1_foff.as<unsigned long long>(), a->src_frames, a->d_foff.as<unsigned long long>(),
                                                    a->P.n_frames, a->idb == 4 ? 1u : 0u, mb.v1_send.as<uint32_t>(), a->d_ctr.as<Counters>());
@@ -866,7 +887,7 @@ static int merge_store_update(pa_merge* g) {
     MCK(cudaSetDevice(a->device));
     MergeBufs& mb = g->mb[i];
     if (++a->store_epoch >= (1ull << 32)) return g->fail(a->fail(PA_ERANGE, "stack store: access clock overflow"), a->err);
-    a->store_frames_sent = 0;
+    a->store_frames_sent = 0; a->store_refs_sent = 0;
     MCK(mb.v1_last.ensure(std::max<uint64_t>(U, 1) * 4));
     MCK(cudaMemsetAsync(mb.v1_last.p, 0xFF, U * 4, a->s_comp));
     k_merged_last_rows<<<a->G, kThreads, 0, a->s_comp>>>((uint32_t)a->N, a->d_slot.as<uint32_t>(), a->d_table.as<StackSlot>(), (uint32_t)a->P.row_base, mb.v1_last.as<uint32_t>());
@@ -908,7 +929,8 @@ static int merge_store_update(pa_merge* g) {
       StoreInsertArgs sa = store_insert_args(a, min_last_p1);
       sa.gtab = mb.gtab.as<StackSlot>(); sa.g_slot = mb.g_uniq_slot.as<uint32_t>(); sa.g_last_inv = last[i];
       sa.g_frames = mb.v1_frames.as<uint32_t>(); sa.g_foff = mb.v1_foff.as<unsigned long long>();
-      k_store_insert<true><<<a->G, kThreads, 0, a->s_comp>>>(sa);
+      if (g->group_stacks) { sa.g_refs = mb.v1_frames.as<unsigned long long>(); k_store_insert<true, true><<<a->G, kThreads, 0, a->s_comp>>>(sa); }
+      else k_store_insert<true><<<a->G, kThreads, 0, a->s_comp>>>(sa);
       MCK(cudaMemcpyAsync(a->h_ctr_pinned, ctr, sizeof(Counters), cudaMemcpyDeviceToHost, a->s_comp));
       if ((rc = store_ctl_read(a, &ctl))) return g->fail(rc, a->err);
       MCK(cudaGetLastError());
@@ -974,15 +996,15 @@ static int merge_process(pa_merge* g) {
   StreamShare share(g);
   auto restore = [] {};
   // ---- rows of every shard -> global row ranges; registrations must be identical (ids are global)
-  struct Dims { uint64_t n, nf, store_entries, store_frames; uint32_t ncols, nlab, n_frames, n_cstr, n_labelsets, n_funcs, lz4, schema; };
+  struct Dims { uint64_t n, nf, store_entries, store_frames, n_stack_frames, stack_digest; uint32_t ncols, nlab, n_frames, n_cstr, n_labelsets, n_funcs, lz4, schema, group_stacks, n_stacks; };
   std::vector<const void*> src(L);
   std::vector<uint8_t> hb;
   rc = PA_OK;
   for (size_t i = 0; i < L && !rc; i++) {
     pa_agg* a = g->members[i];
     cudaSetDevice(a->device);
-    Dims d{a->N, a->NF, a->store_entries, a->store_frames, (uint32_t)a->cols.size(), a->n_label_cols, a->P.n_frames, a->P.n_cstr, a->P.n_labelsets, a->P.n_funcs,
-           g->lz4 ? 1u : 0u, (uint32_t)a->cfg.schema};
+    Dims d{a->N, a->NF, a->store_entries, a->store_frames, a->P.n_stack_frames, a->P.stack_digest, (uint32_t)a->cols.size(), a->n_label_cols, a->P.n_frames,
+           a->P.n_cstr, a->P.n_labelsets, a->P.n_funcs, g->lz4 ? 1u : 0u, (uint32_t)a->cfg.schema, a->group_stacks ? 1u : 0u, a->P.n_stacks};
     if (g->mb[i].gather_scratch.ensure(std::max<size_t>((size_t)(W + 1) * sizeof(Dims), 256)) != cudaSuccess) { rc = g->fail(PA_ENOMEM, "device allocation failed"); break; }
     // staged through the tail of the gather scratch (the head receives the gathered block)
     uint8_t* mine = g->mb[i].gather_scratch.as<uint8_t>() + (size_t)W * sizeof(Dims);
@@ -995,12 +1017,21 @@ static int merge_process(pa_merge* g) {
   for (uint32_t r = 0; r < W; r++) {  // one member per process: the group's modes are settled here, before any work
     if (dims[r].lz4 != dims[0].lz4) { restore(); return g->fail(PA_EINVAL, kLz4Mixed); }
     if (dims[r].schema != dims[0].schema) { restore(); return g->fail(PA_EINVAL, kSchemaMixed); }
+    const char* why = dims[r].group_stacks != dims[0].group_stacks ? kStacksMixed
+                    : dims[0].group_stacks && (dims[r].n_stacks != dims[0].n_stacks || dims[r].n_stack_frames != dims[0].n_stack_frames ||
+                                               dims[r].stack_digest != dims[0].stack_digest) ? kStacksMismatch : nullptr;
+    if (why) {  // (also where the caller of each local member looks for it)
+      restore();
+      for (pa_agg* m : g->members) m->fail(PA_EINVAL, why);
+      return g->fail(PA_EINVAL, why);
+    }
     if (dims[0].schema == PA_SCHEMA_V1 && (dims[r].store_entries != dims[0].store_entries || dims[r].store_frames != dims[0].store_frames)) {
       restore();
       return g->fail(PA_EINVAL, kStoreMismatch);
     }
   }
   const bool v1 = dims[0].schema == PA_SCHEMA_V1;
+  g->group_stacks = dims[0].group_stacks != 0;
   g->n_rows.assign(W, 0); g->nf.assign(W, 0); g->row_base.assign(W + 1, 0);
   g->NT = 0; g->NFT = 0;
   for (uint32_t r = 0; r < W; r++) {
@@ -1012,12 +1043,15 @@ static int merge_process(pa_merge* g) {
     }
   }
   g->row_base[W] = g->NT;
+  // group stacks: the rings hold no frames; the merged location-index stream, and each shard's slice of it, is bounded by the
+  // (identical) registered arena, as one registered-stacks aggregator's is
+  if (g->group_stacks) g->NFT = dims[0].n_stack_frames;
   g->ncols = dims[0].ncols;
   if (g->NT > 0x7FFFFFFFull) { restore(); return g->fail(PA_ERANGE, "merged batch exceeds the int32 row limit of run ends / ListView offsets"); }
   if (g->NT == 0) {  // (like one aggregator's empty batch: no access to the store)
     for (size_t i = 0; i < L; i++) {
       pa_agg* a = g->members[i];
-      a->processed = true; a->last_unique = 0; a->store_frames_sent = 0;
+      a->processed = true; a->last_unique = 0; a->store_frames_sent = 0; a->store_refs_sent = 0;
       memset(&a->h_ctr, 0, sizeof(Counters));
     }
     restore();
@@ -1608,9 +1642,9 @@ static int merge_stacktraces(pa_merge* g, const uint8_t* ids, uint64_t n, pa_agg
 // ---------------------------------------------------------------------------------------------------------------------
 extern "C" {
 
-// registered-stacks members are not supported by merge groups yet (the reason goes into the member's last error)
+// registered-stacks members join merge groups only with group-wide stack ids (the reason goes into the member's last error)
 static bool refuse_registered(pa_agg* m) {
-  if (!m->registered) return false;
+  if (!m->registered || m->group_stacks) return false;
   m->fail(PA_EINVAL, "merge groups do not support PA_CFG_REGISTERED_STACKS members yet");
   return true;
 }
@@ -1623,7 +1657,12 @@ int pa_merge_create_local(pa_agg* const* members, uint32_t n, pa_merge** out) {
     n_lz4 += lz4_gpu_member(members[i]);
   }
   bool any_registered = false;
-  for (uint32_t i = 0; i < n; i++) any_registered |= refuse_registered(members[i]);
+  uint32_t n_stacks = 0;
+  for (uint32_t i = 0; i < n; i++) { any_registered |= refuse_registered(members[i]); n_stacks += group_stacks_member(members[i]); }
+  if (n_stacks && n_stacks != n) {  // (the reason goes into every member's last error; a plain registered member keeps its own)
+    for (uint32_t i = 0; i < n; i++) if (!members[i]->registered || members[i]->group_stacks) members[i]->fail(PA_EINVAL, kStacksMixed);
+    return PA_EINVAL;
+  }
   if (any_registered) return PA_EINVAL;
   if (n_lz4 && n_lz4 != n) {  // the reason goes where the caller of a PA_IPC_LZ4_FRAME_GPU member looks for it
     for (uint32_t i = 0; i < n; i++) if (lz4_gpu_member(members[i])) members[i]->fail(PA_EINVAL, kLz4Mixed);

@@ -433,6 +433,44 @@ def stack_form(w):
     return StackForm(np.asarray(hashes, dtype=np.uint64).reshape(-1, 2), frames, offsets, of_row)
 
 
+def group_stack_form(parts):
+    """PA_CFG_GROUP_STACKS: (one StackForm over the union of the parts' stacks, [each part's stack_of_row in it]). Every member
+    of a merge group registers that form, so a row names the same stack on every shard; in PA_HASH_PROVIDED mode a stack's id
+    comes from whichever part's rows name it. The form's own stack_of_row is that of the concatenated parts (one aggregator fed
+    [part 0's rows, part 1's rows, ...])."""
+    parts = list(parts)
+    t0 = parts[0].stack_table if parts else None
+    if parts and all(p._frame_ids is None and (p.stack_table is t0 or np.array_equal(p.stack_table, t0)) for p in parts):
+        t = np.ascontiguousarray(t0, dtype=np.uint64)  # one shared stack table: register it once
+        hashes = np.zeros((t.shape[0], 2), dtype=np.uint64)
+        for p in parts:
+            hashes[p.stack_choice, 0] = p.hdrs["hash_hi"]
+            hashes[p.stack_choice, 1] = p.hdrs["hash_lo"]
+        offsets = np.arange(t.shape[0] + 1, dtype=np.uint64) * np.uint64(t.shape[1])
+        rows = [np.asarray(p.stack_choice, dtype=np.uint64) for p in parts]
+        return StackForm(hashes, t.reshape(-1), offsets, np.concatenate(rows)), rows
+    index, hashes, stacks, rows = {}, [], [], []
+    for p in parts:  # each part's own stacks, deduplicated across the parts on (hash_hi, hash_lo, frame ids) as stack_form does
+        sf = stack_form(p)
+        offs = sf.offsets.astype(np.int64)
+        remap = np.zeros(len(offs) - 1, dtype=np.uint64)
+        for s, (hi, lo) in enumerate(sf.hashes.tolist()):
+            fr = np.asarray(sf.frames[offs[s]:offs[s + 1]], dtype=np.uint64)
+            key = (hi, lo, fr.tobytes())
+            g = index.get(key)
+            if g is None:
+                g = index[key] = len(stacks)
+                hashes.append((hi, lo))
+                stacks.append(fr)
+            remap[s] = g
+        rows.append(remap[np.asarray(sf.stack_of_row, dtype=np.int64)])
+    offsets = np.zeros(len(stacks) + 1, dtype=np.uint64)
+    offsets[1:] = np.cumsum([len(f) for f in stacks], dtype=np.uint64)
+    frames = np.concatenate(stacks) if stacks else np.zeros(0, np.uint64)
+    of_row = np.concatenate(rows) if rows else np.zeros(0, np.uint64)
+    return StackForm(np.asarray(hashes, dtype=np.uint64).reshape(-1, 2), frames, offsets, of_row), rows
+
+
 def expand_stack_form(hdrs, sf):
     """The ring form of rows in registered-stacks form: (headers with hash_hi / hash_lo / nframes / frame_off of their stack,
     concatenated frame ids) — what an aggregator without PA_CFG_REGISTERED_STACKS ingests for the same samples."""
@@ -451,16 +489,19 @@ def expand_stack_form(hdrs, sf):
     return hd, np.asarray(sf.frames, dtype=np.uint64)[idx]
 
 
-def from_workload(w, device=0, max_samples=None, max_frames=None, chunk_samples=0, registered_stacks=False, flags=0, **kw):
+def from_workload(w, device=0, max_samples=None, max_frames=None, chunk_samples=0, registered_stacks=False, group_form=None, flags=0, **kw):
     """Aggregator with the workload's dictionaries registered (string id 0 == "" is implicit). registered_stacks: a
     PA_CFG_REGISTERED_STACKS aggregator with the workload's stacks registered too (stack_form); max_frames then defaults to
-    the registered frames."""
-    sf = stack_form(w) if registered_stacks else None
+    the registered frames. group_form: a PA_CFG_REGISTERED_STACKS | PA_CFG_GROUP_STACKS aggregator that registers this
+    StackForm (group_stack_form) instead, as every member of its merge group does."""
+    sf = group_form if group_form is not None else stack_form(w) if registered_stacks else None
+    if group_form is not None:
+        flags |= abi.PA_CFG_REGISTERED_STACKS | abi.PA_CFG_GROUP_STACKS
     n = max(1, w.n if max_samples is None else max_samples)
     nf = max(1, (len(sf.frames) if sf else w.n_frame_ids) if max_frames is None else max_frames)
     a = Aggregator(device=device, hash_mode=w.hash_mode, label_flags=w.label_flags, samples_per_second=w.samples_per_second,
                    external_labels=w.external_labels, max_samples=n, max_frames=nf, chunk_samples=chunk_samples, schema=getattr(w, "schema", 0),
-                   flags=flags | (abi.PA_CFG_REGISTERED_STACKS if registered_stacks else 0), **kw)
+                   flags=flags | (abi.PA_CFG_REGISTERED_STACKS if sf is not None else 0), **kw)
     first = a.register_strings(w.strings[1:])
     assert first == 1, first
     a.register_frames(w.frames)
@@ -474,7 +515,8 @@ def from_workload(w, device=0, max_samples=None, max_frames=None, chunk_samples=
 def load(a, w, stack_of_row=None):
     """Write the workload's rows straight into the pinned ring (no intermediate copy of the frame stream). On a registered-stacks
     aggregator the rows name registered stacks (stack_of_row, by default those from_workload(w, registered_stacks=True)
-    registered) and the ring gets no frames."""
+    registered) and the ring gets no frames; a merge group member fed one part of a group_stack_form takes that part's
+    stack_of_row."""
     if a.registered:
         hv, _, _ = a.acquire(w.n, 0)
         hv[:] = w.hdrs

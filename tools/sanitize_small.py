@@ -2,7 +2,7 @@
 added in round 2 — early copy-out during a multi-chunk flush, the v1 LRU store (evictions, revivals, compaction, over-full batch),
 the pipelined / bulk-copy-staged hash variants, the narrow ring, a 3-shard merged record.
 
-usage: PA_EARLY_D2H_ALWAYS=1 compute-sanitizer --tool memcheck python tools/sanitize_small.py [plain|lz4_gpu|merge_lz4_gpu]
+usage: PA_EARLY_D2H_ALWAYS=1 compute-sanitizer --tool memcheck python tools/sanitize_small.py [plain|lz4_gpu|merge_lz4_gpu|merge_v1|registered|merge_group_stacks]
 lz4_gpu: small flushes with the bodies compressed on the device (PA_IPC_LZ4_FRAME_GPU) instead: a multi-chunk v2 batch, the
 narrow ring, and a v1 batch with its stacktrace record, each checked against the oracle's plain stream.
 merge_lz4_gpu: a small in-process merge group of PA_IPC_LZ4_FRAME_GPU members whose shard cuts put blocks across part borders
@@ -10,7 +10,10 @@ merge_lz4_gpu: a small in-process merge group of PA_IPC_LZ4_FRAME_GPU members wh
 merge_v1: in-process groups of PA_SCHEMA_V1 members over several intervals against a small store (evictions, compaction, an
 over-full batch, stacktrace requests), plain and PA_IPC_LZ4_FRAME_GPU, checked against one v1 aggregator and the oracle.
 registered: PA_CFG_REGISTERED_STACKS aggregators (both hash modes, the narrow ring, small chunks, v1) against the oracle, and a
-row naming an unregistered stack id followed by a clean flush."""
+row naming an unregistered stack id followed by a clean flush.
+merge_group_stacks: in-process groups of PA_CFG_GROUP_STACKS members — a v2 interval over three shards with an empty one, and
+v1 intervals against a small store (stack references instead of frames), checked against one group-stacks aggregator, a ring
+group and the oracle."""
 import os
 import sys
 
@@ -103,8 +106,19 @@ def registered():
     print("sanitize_small registered ok")
 
 
+def merge_group_stacks():
+    from test_merge_group_stacks import lru_quad, one_interval
+    w = synth.edge_workload(seed=5, n=2000, hash_mode=abi.PA_HASH_PROVIDED, external=False)
+    idx = sharded.shard_rows(w, 2)
+    one_interval(oracle_py, lib, w, [idx[0], np.zeros(0, np.int64), idx[1]])
+    lru_quad(oracle_py, lib, 3, intervals=4).close()
+    print("sanitize_small merge_group_stacks ok")
+
+
 def main():
     oracle_py.build()
+    if sys.argv[1:] == ["merge_group_stacks"]:
+        return merge_group_stacks()
     if sys.argv[1:] == ["registered"]:
         return registered()
     if sys.argv[1:] == ["lz4_gpu"]:
