@@ -100,6 +100,17 @@ enum {
                                     rank when they differ. A group cannot mix such members with ring members (pa_merge_create_local
                                     refuses it, multi-process groups fail pa_merge_process on every rank). On its own the aggregator
                                     behaves exactly like a PA_CFG_REGISTERED_STACKS one */
+#define PA_CFG_RETIRE_STACKS 0x8u /* with PA_CFG_REGISTERED_STACKS only, and not with PA_CFG_GROUP_STACKS (pa_agg_create fails with
+                                    PA_EINVAL otherwise): registered stacks that no batch has named for a while can be retired
+                                    (pa_agg_retire_stacks) and their slots reused, so the registry of a long-running agent stays bounded.
+                                    A stack is named by a 64-bit handle, generation << 32 | slot, that pa_agg_register_stack_handles
+                                    returns; a row puts it in frame_off. A slot that was never reused has generation 0, so its handle is
+                                    the id the plain mode would have given. A handle whose slot has been freed or reused never names
+                                    another stack: a row that carries one fails its flush with PA_EINVAL (the next flush works).
+                                    pa_agg_register_stacks is refused (PA_EINVAL). max_frames bounds the frames of the stacks not yet
+                                    freed (live, pending, and retired ones still in their grace batch); the frames freed stacks leave
+                                    behind do not count, and the device arena is compacted when they outweigh the live ones. The
+                                    output is byte for byte the same as without the flag */
 
 #define PA_NO_STRING 0xFFFFFFFFu /* "no value"; string id 0 is always the empty string "" */
 
@@ -226,6 +237,23 @@ int pa_agg_register_labelsets(pa_agg* a, const pa_label_pair* pairs, const uint3
  * PA_EINVAL: unregistered frame id, aggregator without the flag, hashes given / missing for the hash mode.
  * PA_ERANGE: a stack deeper than 65535. PA_ENOSPC: the registered frames would exceed max_frames. */
 int pa_agg_register_stacks(pa_agg* a, const uint64_t* hashes, const uint64_t* frames, const uint64_t* offsets, uint32_t n, uint64_t* first_stack_id);
+/* The same inputs, validation and errors as pa_agg_register_stacks, in either registered mode; handles[i] receives the handle of
+ * stack i (n entries). Without PA_CFG_RETIRE_STACKS the handles are the consecutive ids. With it, a stack takes the lowest free
+ * slot (with that slot's next generation) or else a new slot, so the handles need not be consecutive. */
+int pa_agg_register_stack_handles(pa_agg* a, const uint64_t* hashes, const uint64_t* frames, const uint64_t* offsets, uint32_t n, uint64_t* handles);
+/* PA_CFG_RETIRE_STACKS only. Call it between flushes, from the flushing thread (ingest and registration may run meanwhile);
+ * PA_EINVAL while a staged batch has not been collected, for idle_batches == 0, and on other aggregators.
+ * Retires every live stack that is idle for idle_batches batches: registered before the last idle_batches batches were staged,
+ * and named by none of them. At most `cap` are retired, lowest slot first; their handles go to handles[] in ascending slot order
+ * and their count to *n_retired. Idle stacks beyond `cap` stay live; a later call finds them.
+ * Grace rule: rows of the NEXT batch may still name a retired stack and come out exactly right (rows a producer committed before
+ * the caller forgot the handle). The stack is freed when the batch after that one is staged; from then on its slot may go to a new
+ * registration. The caller drops the returned handles from its own lookup before its next flush.
+ * Counters through pa_agg_last_kernel_ms (in *launches, ms = 0, saturating at 2^32 - 1): "stacks_live" (registered and not yet
+ * freed), "stacks_free" (free slots), "stack_frames_live" (their frames), "stack_frames_dead" (frames of freed stacks still in the
+ * device arena), "stack_compactions" and "stacks_retired" (since creation). "stack_compact" reports the device time (ms) and kernel
+ * launches of the last arena compaction. These names fail with PA_EINVAL on aggregators without PA_CFG_RETIRE_STACKS. */
+int pa_agg_retire_stacks(pa_agg* a, uint32_t idle_batches, uint64_t* handles, uint64_t cap, uint64_t* n_retired);
 
 /* ingest — ReportTraceEvent (:219). Thread-safe; row order == acquisition order (the mutex at :335).
  * acquire reserves space for n_rows headers / n_frames frame ids in the pinned ring and returns

@@ -192,6 +192,22 @@ struct pa_agg {
   std::vector<uint32_t> reg_arena;
   Mirror<RegStack> m_stacks;
   Mirror<uint32_t> m_arena;
+  // PA_CFG_RETIRE_STACKS: the device holds the registry (records, last_use, the frame arena). The host keeps per-slot metadata,
+  // the free slots (a min-heap), the retired stacks waiting for their grace batch, and the registrations not yet uploaded.
+  enum : uint8_t { RS_LIVE, RS_RETIRING, RS_FREE };
+  bool retire = false;
+  std::vector<uint32_t> rs_depth, rs_gen;  // rs_gen: the generation of the slot's current (or next) stack
+  std::vector<uint8_t> rs_state;
+  std::vector<uint32_t> rs_free;
+  std::vector<std::pair<uint32_t, uint64_t>> rs_retiring;  // (slot, stage count at which it is freed)
+  std::vector<RegStack> rs_pend;  // off relative to rs_pend_frames
+  std::vector<uint32_t> rs_pend_slot, rs_pend_seq, rs_pend_frames;
+  uint64_t rs_stages = 0;         // batches staged so far (the sequence number of the last one)
+  uint64_t rs_live = 0, rs_frames_live = 0, rs_frames_dead = 0, rs_retired = 0, rs_compactions = 0;
+  uint64_t rs_dev_slots = 0, rs_dev_len = 0;  // records and arena ids on the device (dead frames included)
+  DBuf d_rs_recs, d_rs_last, d_rs_arena[2], d_rs_tmp, d_rs_upd;
+  int rs_cur = 0;
+  Timer rs_tm;  // the last compaction
   // v1: frames resolved by the buildStacktraceRecord rules + the device-resident store of known stacks
   Mirror<uint32_t> m1_map, m1_bid, m1_fn, m1_file;
   Mirror<uint64_t> m1_line, m1_col;
@@ -391,6 +407,7 @@ int pa_agg_create(const pa_agg_config* cfg, pa_agg** out) {
   if (!cfg || !out || cfg->abi_version != PA_ABI_VERSION || cfg->samples_per_second == 0 || cfg->max_samples == 0 || cfg->hash_mode > 1 || cfg->schema > 1 || cfg->ipc_compression > PA_IPC_LZ4_FRAME_GPU ||
       (cfg->frame_id_bytes != 0 && cfg->frame_id_bytes != 4 && cfg->frame_id_bytes != 8)) return PA_EINVAL;
   if ((cfg->flags & PA_CFG_GROUP_STACKS) && !(cfg->flags & PA_CFG_REGISTERED_STACKS)) return PA_EINVAL;
+  if ((cfg->flags & PA_CFG_RETIRE_STACKS) && (!(cfg->flags & PA_CFG_REGISTERED_STACKS) || (cfg->flags & PA_CFG_GROUP_STACKS))) return PA_EINVAL;
   if (cfg->max_samples > 0x7FFFFFFFull) return PA_ERANGE;  // run ends / ListView offsets are int32
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || cfg->device < 0 || cfg->device >= ndev) return PA_ENODEV;
@@ -403,6 +420,7 @@ int pa_agg_create(const pa_agg_config* cfg, pa_agg** out) {
   a->single_ring = (cfg->flags & PA_CFG_SINGLE_RING) != 0;
   a->registered = (cfg->flags & PA_CFG_REGISTERED_STACKS) != 0;
   a->group_stacks = (cfg->flags & PA_CFG_GROUP_STACKS) != 0;
+  a->retire = (cfg->flags & PA_CFG_RETIRE_STACKS) != 0;
   auto bail = [&](int code) { pa_agg_destroy(a); return code; };
   if (cudaSetDevice(a->device) != cudaSuccess) return bail(PA_ENODEV);
   cudaDeviceProp prop;
@@ -464,6 +482,7 @@ int pa_agg_create(const pa_agg_config* cfg, pa_agg** out) {
   cudaEventCreate(&a->ev_d2h0);
   cudaEventCreate(&a->ev_d2h1);
   for (int t = 0; t < T_COUNT; t++) { cudaEventCreate(&a->tm[t].a); cudaEventCreate(&a->tm[t].b); }
+  if (a->retire) { cudaEventCreate(&a->rs_tm.a); cudaEventCreate(&a->rs_tm.b); }
   if (a->cfg.ipc_compression == PA_IPC_LZ4_FRAME_GPU) { cudaEventCreate(&a->ev_lz4p0); cudaEventCreate(&a->ev_lz4p1); }
   const uint64_t N = a->cfg.max_samples, NF = a->cfg.max_frames;
   if (a->idb == 4 && a->hash_variant != 5) a->hash_variant = 2;  // (the tma variants fall through to wide32 in launch_hash)  // the narrow ring is read by the `wide` kernel (widening loads); the other variants take uint64 ids
@@ -534,7 +553,8 @@ void pa_agg_destroy(pa_agg* a) {
                  &a->d_arena, &a->d_partial, &a->d_partial2, &a->d_ree_partial, &a->d_lsmat, &a->d_kindtab, &a->d_cols, &a->d_jobs,
                  &a->m_stacks.buf, &a->m_arena.buf, &a->m_addr.buf, &a->m_line.buf, &a->m_type.buf, &a->m_map.buf, &a->m_bid.buf, &a->m_func.buf, &a->m_fnfile.buf, &a->m_sid2cid.buf,
                  &a->m1_map.buf, &a->m1_bid.buf, &a->m1_fn.buf, &a->m1_file.buf, &a->m1_line.buf, &a->m1_col.buf, &a->m1_complete.buf,
-                 &a->d_store, &a->d_store_arena, &a->d_store_ctl, &a->d_v1_ids, &a->d_st1, &a->d_store_stamp, &a->d_v1_last, &a->d_select, &a->d_lz4, &a->d_lz4_body};
+                 &a->d_store, &a->d_store_arena, &a->d_store_ctl, &a->d_v1_ids, &a->d_st1, &a->d_store_stamp, &a->d_v1_last, &a->d_select, &a->d_lz4, &a->d_lz4_body,
+                 &a->d_rs_recs, &a->d_rs_last, &a->d_rs_arena[0], &a->d_rs_arena[1], &a->d_rs_tmp, &a->d_rs_upd};
   for (DBuf* b : all) b->release();
   for (auto e : a->chunk_ev) cudaEventDestroy(e);
   if (a->ev_h2d0) cudaEventDestroy(a->ev_h2d0);
@@ -544,6 +564,8 @@ void pa_agg_destroy(pa_agg* a) {
   if (a->ev_lz4p0) cudaEventDestroy(a->ev_lz4p0);
   if (a->ev_lz4p1) cudaEventDestroy(a->ev_lz4p1);
   for (int t = 0; t < T_COUNT; t++) { if (a->tm[t].a) cudaEventDestroy(a->tm[t].a); if (a->tm[t].b) cudaEventDestroy(a->tm[t].b); }
+  if (a->rs_tm.a) cudaEventDestroy(a->rs_tm.a);
+  if (a->rs_tm.b) cudaEventDestroy(a->rs_tm.b);
   if (a->ev_fork) cudaEventDestroy(a->ev_fork);
   if (a->ev_join) cudaEventDestroy(a->ev_join);
   if (a->s_copy2) { cudaStreamSynchronize(a->s_copy2); cudaStreamDestroy(a->s_copy2); }
@@ -590,30 +612,66 @@ int pa_agg_register_labelsets(pa_agg* a, const pa_label_pair* pairs, const uint3
   a->cols_dirty = true;
   return PA_OK;
 }
-int pa_agg_register_stacks(pa_agg* a, const uint64_t* hashes, const uint64_t* frames, const uint64_t* offsets, uint32_t n, uint64_t* first_stack_id) {
-  if (!a) return PA_EINVAL;
-  if (!a->registered) return a->fail(PA_EINVAL, "pa_agg_register_stacks needs an aggregator created with PA_CFG_REGISTERED_STACKS");
+// Validation shared by both registration calls (a refused call registers nothing). check_stack_args runs before reg_mu is
+// taken, check_stack_shape and check_stack_frames under it, with the mode's space check in between.
+static int check_stack_args(pa_agg* a, const uint64_t* hashes, const uint64_t* offsets, uint32_t n, const char* fn) {
+  if (!a->registered) return a->fail(PA_EINVAL, (std::string(fn) + " needs an aggregator created with PA_CFG_REGISTERED_STACKS").c_str());
   if (n && !offsets) return PA_EINVAL;
   const bool provided = a->cfg.hash_mode == PA_HASH_PROVIDED;
   if (n && provided && !hashes) return a->fail(PA_EINVAL, "PA_HASH_PROVIDED: register_stacks needs the stack ids (hashes)");
   if (!provided && hashes) return a->fail(PA_EINVAL, "PA_HASH_XXH64X2: the library computes the stack ids (hashes must be NULL)");
-  std::lock_guard<std::mutex> g(a->reg_mu);
-  const uint64_t nf_reg = a->ft.count(), words = a->idb / 4;
-  const uint64_t have = a->reg_arena.size() / words;
+  return PA_OK;
+}
+static int check_stack_shape(pa_agg* a, const uint64_t* frames, const uint64_t* offsets, uint32_t n, uint64_t* total_out) {
   uint64_t total = 0;
-  for (uint32_t i = 0; i < n; i++) {  // validate everything first: a refused call registers nothing
+  for (uint32_t i = 0; i < n; i++) {
     if (offsets[i + 1] < offsets[i]) return a->fail(PA_EINVAL, "stack offsets must be non-decreasing");
     const uint64_t d = offsets[i + 1] - offsets[i];
     if (d > 0xFFFFu) return a->fail(PA_ERANGE, "stack deeper than 65535 frames");
     total += d;
   }
   if (total && !frames) return PA_EINVAL;
-  if (have + total > a->cfg.max_frames) return a->fail(PA_ENOSPC, "registered frames would exceed max_frames");
-  if (a->reg_stacks.size() + n > 0xFFFFFFFFull) return a->fail(PA_ENOSPC, "more than 2^32 - 1 registered stacks");  // (ids are checked as uint32 on the device)
+  *total_out = total;
+  return PA_OK;
+}
+static int check_stack_frames(pa_agg* a, const uint64_t* frames, const uint64_t* offsets, uint32_t n) {
+  const uint64_t nf_reg = a->ft.count();
   const uint32_t* f32 = (const uint32_t*)frames;
   for (uint32_t i = 0; i < n; i++)
     for (uint64_t j = offsets[i]; j < offsets[i + 1]; j++)
       if ((a->idb == 4 ? (uint64_t)f32[j] : frames[j]) >= nf_reg) return a->fail(PA_EINVAL, "stack refers to an unregistered frame id");
+  return PA_OK;
+}
+// the stack id of stack i: given (PA_HASH_PROVIDED) or, as for a ring row with these frames (DESIGN section 3), XXH64 over the
+// ids as little-endian uint64
+static void stack_key(const pa_agg* a, const uint64_t* hashes, const uint64_t* frames, const uint64_t* offsets, uint32_t i, RegStack* s, std::vector<uint64_t>& wide) {
+  if (a->cfg.hash_mode == PA_HASH_PROVIDED) {
+    s->hash_hi = hashes[2 * i];
+    s->hash_lo = hashes[2 * i + 1];
+    return;
+  }
+  const uint64_t d = offsets[i + 1] - offsets[i];
+  const uint32_t* f32 = (const uint32_t*)frames;
+  wide.resize(d);
+  for (uint64_t j = 0; j < d; j++) wide[j] = a->idb == 4 ? (uint64_t)f32[offsets[i] + j] : frames[offsets[i] + j];
+  s->hash_hi = pa_xxh64(wide.data(), d * 8, 0);
+  s->hash_lo = pa_xxh64(wide.data(), d * 8, PA_XXH_SEED_LO);
+}
+
+int pa_agg_register_stacks(pa_agg* a, const uint64_t* hashes, const uint64_t* frames, const uint64_t* offsets, uint32_t n, uint64_t* first_stack_id) {
+  if (!a) return PA_EINVAL;
+  int rc = check_stack_args(a, hashes, offsets, n, "pa_agg_register_stacks");
+  if (rc) return rc;
+  if (a->retire) return a->fail(PA_EINVAL, "PA_CFG_RETIRE_STACKS: register through pa_agg_register_stack_handles");
+  std::lock_guard<std::mutex> g(a->reg_mu);
+  const uint64_t words = a->idb / 4;
+  const uint64_t have = a->reg_arena.size() / words;
+  uint64_t total = 0;
+  if ((rc = check_stack_shape(a, frames, offsets, n, &total))) return rc;
+  if (have + total > a->cfg.max_frames) return a->fail(PA_ENOSPC, "registered frames would exceed max_frames");
+  if (a->reg_stacks.size() + n > 0xFFFFFFFFull) return a->fail(PA_ENOSPC, "more than 2^32 - 1 registered stacks");  // (ids are checked as uint32 on the device)
+  const uint32_t* f32 = (const uint32_t*)frames;
+  if ((rc = check_stack_frames(a, frames, offsets, n))) return rc;
   if (first_stack_id) *first_stack_id = a->reg_stacks.size();
   std::vector<uint64_t> wide;
   for (uint32_t i = 0; i < n; i++) {
@@ -624,15 +682,7 @@ int pa_agg_register_stacks(pa_agg* a, const uint64_t* hashes, const uint64_t* fr
     const uint8_t* src = (const uint8_t*)frames + offsets[i] * a->idb;
     a->reg_arena.resize(a->reg_arena.size() + d * words);
     if (d) memcpy(a->reg_arena.data() + s.off * words, src, d * a->idb);
-    if (provided) {
-      s.hash_hi = hashes[2 * i];
-      s.hash_lo = hashes[2 * i + 1];
-    } else {  // the stack id of a ring row with these frames (DESIGN section 3): XXH64 over the ids as little-endian uint64
-      wide.resize(d);
-      for (uint64_t j = 0; j < d; j++) wide[j] = a->idb == 4 ? (uint64_t)f32[offsets[i] + j] : frames[offsets[i] + j];
-      s.hash_hi = pa_xxh64(wide.data(), d * 8, 0);
-      s.hash_lo = pa_xxh64(wide.data(), d * 8, PA_XXH_SEED_LO);
-    }
+    stack_key(a, hashes, frames, offsets, i, &s, wide);
     if (a->group_stacks) {  // the registry's digest: XXH64 of (hash_hi, hash_lo, depth, frame ids as uint64), seeded with the digest so far
       wide.resize(d + 3);
       wide[0] = s.hash_hi; wide[1] = s.hash_lo; wide[2] = d;
@@ -640,6 +690,49 @@ int pa_agg_register_stacks(pa_agg* a, const uint64_t* hashes, const uint64_t* fr
       a->reg_digest = pa_xxh64(wide.data(), (d + 3) * 8, a->reg_digest);
     }
     a->reg_stacks.push_back(s);
+  }
+  return PA_OK;
+}
+int pa_agg_register_stack_handles(pa_agg* a, const uint64_t* hashes, const uint64_t* frames, const uint64_t* offsets, uint32_t n, uint64_t* handles) {
+  if (!a || (n && !handles)) return PA_EINVAL;
+  if (!a->retire) {
+    uint64_t first = 0;
+    int rc = pa_agg_register_stacks(a, hashes, frames, offsets, n, &first);
+    for (uint32_t i = 0; i < n && !rc; i++) handles[i] = first + i;
+    return rc;
+  }
+  int rc = check_stack_args(a, hashes, offsets, n, "pa_agg_register_stack_handles");
+  if (rc) return rc;
+  std::lock_guard<std::mutex> g(a->reg_mu);
+  uint64_t total = 0;
+  if ((rc = check_stack_shape(a, frames, offsets, n, &total))) return rc;
+  if (a->rs_frames_live + total > a->cfg.max_frames) return a->fail(PA_ENOSPC, "live registered frames would exceed max_frames");
+  if (n > a->rs_free.size() && a->rs_state.size() + (n - a->rs_free.size()) > 0xFFFFFFFFull) return a->fail(PA_ENOSPC, "more than 2^32 - 1 stack slots");
+  if ((rc = check_stack_frames(a, frames, offsets, n))) return rc;
+  const uint64_t words = a->idb / 4;
+  std::vector<uint64_t> wide;
+  for (uint32_t i = 0; i < n; i++) {
+    const uint64_t d = offsets[i + 1] - offsets[i];
+    uint32_t slot;
+    if (!a->rs_free.empty()) {  // the lowest free slot
+      std::pop_heap(a->rs_free.begin(), a->rs_free.end(), std::greater<uint32_t>());
+      slot = a->rs_free.back();
+      a->rs_free.pop_back();
+    } else {
+      slot = (uint32_t)a->rs_state.size();
+      a->rs_state.push_back(pa_agg::RS_FREE); a->rs_depth.push_back(0); a->rs_gen.push_back(0);
+    }
+    RegStack s{};
+    s.off = a->rs_pend_frames.size() / words;
+    s.depth = (uint32_t)d;
+    s.pad = a->rs_gen[slot];
+    stack_key(a, hashes, frames, offsets, i, &s, wide);
+    a->rs_pend_frames.resize(a->rs_pend_frames.size() + d * words);
+    if (d) memcpy(a->rs_pend_frames.data() + s.off * words, (const uint8_t*)frames + offsets[i] * a->idb, d * a->idb);
+    a->rs_pend.push_back(s); a->rs_pend_slot.push_back(slot); a->rs_pend_seq.push_back((uint32_t)a->rs_stages);
+    a->rs_state[slot] = pa_agg::RS_LIVE; a->rs_depth[slot] = (uint32_t)d;
+    a->rs_live++; a->rs_frames_live += d;
+    handles[i] = ((uint64_t)a->rs_gen[slot] << 32) | slot;
   }
   return PA_OK;
 }
@@ -694,6 +787,9 @@ int pa_agg_submit(pa_agg* a, const pa_sample_hdr* hdrs, const uint64_t* frames, 
 
 }  // extern "C"
 
+static int rs_stage(pa_agg* a);
+static void release_staged(pa_agg* a);
+
 // ---------------------------------------------------------------------------------------------
 // stage: swap ring buffers, start the chunked H2D copies
 static int stage_async(pa_agg* a) {
@@ -712,6 +808,10 @@ static int stage_async(pa_agg* a) {
       a->ring[a->active].rows = 0;
       a->ring[a->active].nfr = 0;
     }
+  }
+  if (a->retire) {
+    int rc = rs_stage(a);
+    if (rc) { release_staged(a); return rc; }  // (a CUDA failure: the detached batch is dropped)
   }
   pa_agg::Ring& r = a->ring[buf];
   a->staged = buf;
@@ -797,6 +897,112 @@ static void launch_scan(pa_agg* a, F f, int njobs, Timer& t, int gx, cudaStream_
 // grid for a pass over at most `bound` elements: >= 2048 elements per CTA, never more than the full grid
 static int small_grid(const pa_agg* a, uint64_t bound) { return (int)std::max<uint64_t>(1, std::min<uint64_t>((uint64_t)a->G, (bound + 2047) / 2048)); }
 
+// PA_CFG_RETIRE_STACKS, under reg_mu, on the compute stream: applies `frees` (records with kStackFree, for free_slots), compacts
+// the arena when the dead frames outweigh the live ones (at a stage only: no batch is resident then) or when the pending frames
+// would not fit (a regrow, before the pass that reads the records), then uploads the pending registrations.
+static int rs_upload(pa_agg* a, const std::vector<RegStack>& frees, const std::vector<uint32_t>& free_slots, bool at_stage) {
+  cudaStream_t s = a->s_comp;
+  const uint64_t words = a->idb / 4, n_slots = a->rs_state.size();
+  if (n_slots * sizeof(RegStack) > a->d_rs_recs.cap) {  // more slots than the device arrays hold: regrow them
+    DBuf nr, nl;
+    const size_t want = std::max<size_t>(2 * n_slots, 1024);
+    CK(nr.ensure(want * sizeof(RegStack)));
+    CK(nl.ensure(want * 4));
+    if (a->rs_dev_slots) {
+      CK(cudaMemcpyAsync(nr.p, a->d_rs_recs.p, a->rs_dev_slots * sizeof(RegStack), cudaMemcpyDeviceToDevice, s));
+      CK(cudaMemcpyAsync(nl.p, a->d_rs_last.p, a->rs_dev_slots * 4, cudaMemcpyDeviceToDevice, s));
+    }
+    CK(cudaStreamSynchronize(s));
+    a->d_rs_recs.release(); a->d_rs_last.release();
+    a->d_rs_recs = nr; a->d_rs_last = nl;
+  }
+  RegStack* recs = a->d_rs_recs.as<RegStack>();
+  uint32_t* last = a->d_rs_last.as<uint32_t>();
+  // the record updates go up in one copy: [records][slots][seqs], frees first
+  const uint64_t nf = frees.size(), nr = a->rs_pend.size(), nu = nf + nr;
+  RegStack* du = nullptr;
+  uint32_t *dslot = nullptr, *dseq = nullptr;
+  if (nu) {
+    std::vector<uint8_t> up(nu * (sizeof(RegStack) + 8));
+    RegStack* hu = (RegStack*)up.data();
+    uint32_t* hslot = (uint32_t*)(hu + nu);
+    uint32_t* hseq = hslot + nu;
+    std::copy(frees.begin(), frees.end(), hu); std::copy(a->rs_pend.begin(), a->rs_pend.end(), hu + nf);
+    std::copy(free_slots.begin(), free_slots.end(), hslot); std::copy(a->rs_pend_slot.begin(), a->rs_pend_slot.end(), hslot + nf);
+    std::fill(hseq, hseq + nf, 0u); std::copy(a->rs_pend_seq.begin(), a->rs_pend_seq.end(), hseq + nf);
+    CK(a->d_rs_upd.ensure(up.size()));
+    CK(cudaMemcpyAsync(a->d_rs_upd.p, up.data(), up.size(), cudaMemcpyHostToDevice, s));  // (pageable: the source is consumed on return)
+    du = a->d_rs_upd.as<RegStack>(); dslot = (uint32_t*)(du + nu); dseq = dslot + nu;
+  }
+  if (nf) k_stack_scatter<<<small_grid(a, nf), kThreads, 0, s>>>(du, dslot, dseq, (uint32_t)nf, 0ull, recs, last);
+  const uint64_t pend = a->rs_pend_frames.size() / words;
+  const uint64_t cap = a->d_rs_arena[a->rs_cur].cap / a->idb, live_dev = a->rs_dev_len - a->rs_frames_dead;
+  const bool grow = a->rs_dev_len + pend > cap;
+  if (grow || (at_stage && a->rs_frames_dead > live_dev)) {
+    DBuf& dst = a->d_rs_arena[a->rs_cur ^ 1];
+    CK(dst.ensure(std::max<uint64_t>(grow ? 2 * (live_dev + pend) : cap, 1024) * a->idb));
+    if (a->rs_dev_slots) {
+      const uint32_t ns = (uint32_t)a->rs_dev_slots;
+      const uint64_t max_chunks = ns + live_dev / kCompactChunk + 1;
+      CK(a->d_rs_tmp.ensure(ns * 8 + max_chunks * 8 + 64));
+      unsigned long long* new_off = a->d_rs_tmp.as<unsigned long long>();
+      uint2* chunks = (uint2*)(new_off + ns);
+      Pair* total = (Pair*)(chunks + max_chunks);
+      a->rs_tm.launches = 0;
+      CK(cudaEventRecord(a->rs_tm.a, s));
+      launch_scan(a, StackLiveF{recs, ns, new_off, chunks, total}, 1, a->rs_tm, small_grid(a, ns), s, a->d_partial);
+      k_stack_compact_copy<<<a->G, kThreads, 0, s>>>(total, chunks, recs, new_off, (uint32_t)words, a->d_rs_arena[a->rs_cur].as<uint32_t>(), dst.as<uint32_t>());
+      k_stack_rebase<<<small_grid(a, ns), kThreads, 0, s>>>(recs, ns, new_off);
+      a->rs_tm.launches += 2;
+      CK(cudaEventRecord(a->rs_tm.b, s));
+      CK(cudaEventSynchronize(a->rs_tm.b));
+      float ms = 0;
+      cudaEventElapsedTime(&ms, a->rs_tm.a, a->rs_tm.b);
+      a->rs_tm.ms = ms;
+      a->rs_compactions++;
+    }
+    a->rs_cur ^= 1;
+    a->rs_dev_len = live_dev;
+    a->rs_frames_dead = 0;
+  }
+  if (nr) {
+    if (pend) CK(cudaMemcpyAsync(a->d_rs_arena[a->rs_cur].as<uint32_t>() + a->rs_dev_len * words, a->rs_pend_frames.data(), pend * a->idb, cudaMemcpyHostToDevice, s));
+    k_stack_scatter<<<small_grid(a, nr), kThreads, 0, s>>>(du + nf, dslot + nf, dseq + nf, (uint32_t)nr, a->rs_dev_len, recs, last);
+    a->rs_dev_len += pend;
+    a->rs_pend.clear(); a->rs_pend_slot.clear(); a->rs_pend_seq.clear(); a->rs_pend_frames.clear();
+  }
+  CK(cudaGetLastError());
+  a->rs_dev_slots = n_slots;
+  a->src_frames = (const unsigned long long*)a->d_rs_arena[a->rs_cur].p;
+  a->P.n_stacks = (uint32_t)n_slots;
+  a->P.n_stack_frames = a->rs_dev_len;
+  return PA_OK;
+}
+
+// A new batch is staged: the stacks whose grace batch this is not (retired before the previous stage) are freed.
+static int rs_stage(pa_agg* a) {
+  std::lock_guard<std::mutex> g(a->reg_mu);
+  a->rs_stages++;
+  std::vector<RegStack> frees;
+  std::vector<uint32_t> slots;
+  size_t keep = 0;
+  for (const auto& e : a->rs_retiring) {
+    if (e.second > a->rs_stages) { a->rs_retiring[keep++] = e; continue; }
+    const uint32_t slot = e.first, d = a->rs_depth[slot];
+    a->rs_state[slot] = pa_agg::RS_FREE;
+    a->rs_live--; a->rs_frames_live -= d; a->rs_frames_dead += d;
+    RegStack r{};
+    r.pad = kStackFree | ++a->rs_gen[slot];
+    frees.push_back(r); slots.push_back(slot);
+    if (a->rs_gen[slot] < kStackFree) {  // (a slot whose 31-bit generation is spent stays free for good)
+      a->rs_free.push_back(slot);
+      std::push_heap(a->rs_free.begin(), a->rs_free.end(), std::greater<uint32_t>());
+    }
+  }
+  a->rs_retiring.resize(keep);
+  return rs_upload(a, frees, slots, true);
+}
+
 static int upload_tables(pa_agg* a) {
   std::lock_guard<std::mutex> g(a->reg_mu);
   cudaStream_t s = a->s_comp;
@@ -808,7 +1014,10 @@ static int upload_tables(pa_agg* a) {
     CK(a->m1_file.sync(a->ft.v1_file_cid, s)); CK(a->m1_line.sync(a->ft.v1_line, s)); CK(a->m1_col.sync(a->ft.v1_col, s));
     CK(a->m1_complete.sync(a->ft.v1_complete, s));
   }
-  if (a->registered) {
+  if (a->retire) {
+    int rc = rs_upload(a, {}, {}, false);
+    if (rc) return rc;
+  } else if (a->registered) {
     CK(a->m_stacks.sync(a->reg_stacks, s)); CK(a->m_arena.sync(a->reg_arena, s));
     a->src_frames = (const unsigned long long*)a->m_arena.ptr();  // (a regrown mirror moves: set on every upload)
     a->P.n_stacks = (uint32_t)a->reg_stacks.size(); a->P.n_stack_frames = a->reg_arena.size() / (a->idb / 4);
@@ -1229,10 +1438,12 @@ static int pass_front(pa_agg* a) {
       if (a->cols[c].type == COL_COMM) h.first_comm = P.col_first[c];
     }
     h.first_kind = P.v1 ? a->v1_first_kind : nullptr;
-    h.stacks = (const uint4*)a->m_stacks.ptr(); h.n_stacks = P.n_stacks;
+    h.stacks = (const uint4*)(a->retire ? a->d_rs_recs.p : a->m_stacks.ptr()); h.n_stacks = P.n_stacks;
+    h.last_use = a->d_rs_last.as<uint32_t>(); h.seq = (uint32_t)a->rs_stages;
     uint64_t rows = r1 - r0;
     int hb = (int)std::min<uint64_t>((rows + kThreads - 1) / kThreads, (uint64_t)a->sms * kHdrBlocksPerSm);
-    if (a->registered) k_header<true><<<std::max(hb, 1), kThreads, 0, s>>>(h);
+    if (a->retire) k_header<true, true><<<std::max(hb, 1), kThreads, 0, s>>>(h);
+    else if (a->registered) k_header<true><<<std::max(hb, 1), kThreads, 0, s>>>(h);
     else k_header<false><<<std::max(hb, 1), kThreads, 0, s>>>(h);
     a->tm[T_HEADER].launches++;
   };
@@ -2616,7 +2827,57 @@ static int shard_export(pa_agg* a, uint64_t frame_base, pa_sample_hdr* hdr_out, 
   return PA_OK;
 }
 
+// PA_CFG_RETIRE_STACKS: idle selection on the device (bitmap, popcount prefix, handles in slot order), then the host marks the
+// retired stacks for freeing at the stage after their grace batch
+static int retire_stacks(pa_agg* a, uint32_t idle, uint64_t* handles, uint64_t cap, uint64_t* n_retired) {
+  if (!a->retire) return a->fail(PA_EINVAL, "pa_agg_retire_stacks needs an aggregator created with PA_CFG_RETIRE_STACKS");
+  if (idle == 0) return a->fail(PA_EINVAL, "idle_batches must be at least 1");
+  if (a->staged >= 0) return a->fail(PA_EINVAL, "collect the staged batch before retiring stacks");
+  if (cap && !handles) return PA_EINVAL;
+  if (n_retired) *n_retired = 0;
+  // rs_stages and rs_dev_slots change only under flush_mu, which this thread holds; stacks registered since the last upload are
+  // not on the device yet and are never idle (their last_use is the current stage count)
+  const uint64_t ns = a->rs_dev_slots;
+  if (a->rs_stages < idle || ns == 0 || cap == 0) return PA_OK;
+  CK(cudaSetDevice(a->device));
+  cudaStream_t s = a->s_comp;
+  const uint32_t nw = (uint32_t)((ns + 31) / 32);
+  const uint64_t nh = std::min<uint64_t>(cap, ns);
+  CK(a->d_rs_tmp.ensure(nh * 8 + 2ull * nw * 4 + 64));
+  unsigned long long* d_handles = a->d_rs_tmp.as<unsigned long long>();
+  uint32_t* bits = (uint32_t*)(d_handles + nh);
+  uint32_t* wprefix = bits + nw;
+  uint32_t* total = wprefix + nw;
+  const RegStack* recs = a->d_rs_recs.as<RegStack>();
+  uint32_t* last = a->d_rs_last.as<uint32_t>();
+  Timer t{};
+  k_stack_idle_bits<<<small_grid(a, ns), kThreads, 0, s>>>(recs, last, (uint32_t)ns, (uint32_t)(a->rs_stages - idle), bits);
+  launch_scan(a, WordsF{bits, wprefix, nw, total}, 1, t, small_grid(a, nw), s, a->d_partial);
+  k_stack_idle_emit<<<small_grid(a, ns), kThreads, 0, s>>>(bits, wprefix, (uint32_t)ns, recs, nh, d_handles, last);
+  uint32_t n_idle = 0;
+  CK(cudaMemcpyAsync(&n_idle, total, 4, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  const uint64_t n = std::min<uint64_t>(n_idle, nh);
+  if (n) CK(cudaMemcpy(handles, d_handles, n * 8, cudaMemcpyDeviceToHost));
+  CK(cudaGetLastError());
+  std::lock_guard<std::mutex> g(a->reg_mu);
+  for (uint64_t i = 0; i < n; i++) {
+    const uint32_t slot = (uint32_t)handles[i];
+    a->rs_state[slot] = pa_agg::RS_RETIRING;
+    a->rs_retiring.emplace_back(slot, a->rs_stages + 2);  // batch rs_stages + 1 is the grace batch
+  }
+  a->rs_retired += n;
+  if (n_retired) *n_retired = n;
+  return PA_OK;
+}
+
 extern "C" {
+
+int pa_agg_retire_stacks(pa_agg* a, uint32_t idle_batches, uint64_t* handles, uint64_t cap, uint64_t* n_retired) {
+  if (!a) return PA_EINVAL;
+  std::lock_guard<std::mutex> g(a->flush_mu);
+  return retire_stacks(a, idle_batches, handles, cap, n_retired);
+}
 
 int pa_agg_shard_sizes(pa_agg* a, uint64_t* n_rows, uint64_t* n_frames) {
   if (!a || !n_rows || !n_frames) return PA_EINVAL;
@@ -2728,6 +2989,25 @@ int pa_agg_last_kernel_ms(const pa_agg* a, const char* name, double* ms, uint32_
   if (!strcmp(name, "store_frames")) {
     if (ms) *ms = 0;
     if (launches) *launches = (uint32_t)std::min<uint64_t>(a->store_frames_sent, 0xFFFFFFFFu);
+    return PA_OK;
+  }
+  // PA_CFG_RETIRE_STACKS (ms is 0): the stack registry's counters
+  {
+    static const char* kRegistryCounters[] = {"stacks_live", "stacks_free", "stack_frames_live", "stack_frames_dead", "stack_compactions", "stacks_retired"};
+    for (int k = 0; k < 6; k++)
+      if (!strcmp(name, kRegistryCounters[k])) {
+        if (!a->retire) return PA_EINVAL;
+        std::lock_guard<std::mutex> g(const_cast<pa_agg*>(a)->reg_mu);
+        const uint64_t v[6] = {a->rs_live, a->rs_state.size() - a->rs_live, a->rs_frames_live, a->rs_frames_dead, a->rs_compactions, a->rs_retired};
+        if (ms) *ms = 0;
+        if (launches) *launches = (uint32_t)std::min<uint64_t>(v[k], 0xFFFFFFFFu);
+        return PA_OK;
+      }
+  }
+  if (!strcmp(name, "stack_compact")) {  // the last arena compaction: device time and launches
+    if (!a->retire) return PA_EINVAL;
+    if (ms) *ms = a->rs_tm.ms;
+    if (launches) *launches = a->rs_tm.launches;
     return PA_OK;
   }
   // PA_SCHEMA_V1 merge groups of PA_CFG_GROUP_STACKS members (ms is 0): stack references (8-byte arena offsets) this member sent

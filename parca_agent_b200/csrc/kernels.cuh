@@ -33,8 +33,9 @@ struct __align__(16) Key128 { unsigned long long hi, lo; };
 struct __align__(32) RegStack {
   unsigned long long hash_hi, hash_lo;  // the stack id, as pa_sample_hdr carries it
   unsigned long long off;
-  uint32_t depth, pad;
+  uint32_t depth, pad;  // PA_CFG_RETIRE_STACKS: pad = the slot's generation, with kStackFree set while the slot is free
 };
+constexpr uint32_t kStackFree = 0x80000000u;
 
 // open-address stack table entry: 32 B = one L2 sector
 struct __align__(32) StackSlot {
@@ -273,6 +274,8 @@ struct HeaderArgs {
   uint32_t* first_kind;          // [8] first row of each sample kind (v1: the kind-derived columns are dictionary encoded)
   const uint4* stacks;           // k_header<true>: the registered stack records (RegStack, two uint4 each)
   uint32_t n_stacks;             // records mirrored for this batch
+  uint32_t* last_use;            // k_header<true, true>: per slot, the sequence number of the last batch that named it
+  uint32_t seq;                  // this batch's sequence number (batches staged so far, this one included)
 };
 
 // Each warp works through tiles of 32 consecutive rows (2 KB of contiguous headers). The next tile's headers arrive in the
@@ -284,9 +287,14 @@ struct HeaderArgs {
 // tables, and forcing the largest carveout made the pass about 30 % slower in provided-hash mode on an H100.
 // kRegistered (PA_CFG_REGISTERED_STACKS): frame_off names a registered stack; its 32-byte record supplies the stack id, the
 // depth and the arena offset, and hash_hi / hash_lo / nframes of the row are ignored. Launched with provided = 1.
+// kRetire (PA_CFG_RETIRE_STACKS): frame_off is a handle, generation << 32 | slot. The record must carry that generation and
+// not be free; the row's batch sequence number is then stored into the slot's last_use word, only when it differs: every row of
+// a batch would write the same value, and with Zipf-distributed stacks the stores to hot slots serialise in L2 (on an H100, each
+// step a new batch of 4M config-3 rows: +0.026 ms of header time over plain registered stacks, +0.235 ms with an unconditional
+// store; DESIGN section 7).
 constexpr int kHdrBlocksPerSm = 8;
 
-template <bool kRegistered>
+template <bool kRegistered, bool kRetire = false>
 __global__ void __launch_bounds__(kThreads, kHdrBlocksPerSm) k_header(HeaderArgs a) {
   __shared__ __align__(128) uint4 tile_buf[kWarps][32 * 4];
   __shared__ __align__(8) unsigned long long tile_bar[kWarps];
@@ -340,7 +348,20 @@ __global__ void __launch_bounds__(kThreads, kHdrBlocksPerSm) k_header(HeaderArgs
       if (ls >= a.n_labelsets) { err |= ERR_BAD_LABELSET; ls = 0; }
       if (comm_sid >= a.n_sids) { err |= ERR_BAD_STRING_ID; comm_sid = 0; }
       if (cpu >= 65536u) { err |= ERR_BAD_CPU; cpu = 0; }
-      if (kRegistered) {
+      if (kRegistered && kRetire) {
+        const uint32_t slot = (uint32_t)foff, gen = (uint32_t)(foff >> 32);
+        uint4 s0{}, s1{};
+        if (slot < a.n_stacks) { s0 = __ldg(a.stacks + 2ull * slot); s1 = __ldg(a.stacks + 2ull * slot + 1); }
+        if (slot < a.n_stacks && s1.w == gen && !(gen & kStackFree)) {
+          k.hi = ((unsigned long long)s0.y << 32) | s0.x;
+          k.lo = ((unsigned long long)s0.w << 32) | s0.z;
+          foff = ((unsigned long long)s1.y << 32) | s1.x;
+          nfr = s1.z;
+          if (a.last_use[slot] != a.seq) a.last_use[slot] = a.seq;
+        } else {
+          err |= ERR_BAD_STACK_ID; k = Key128{0ull, 0ull}; nfr = 0; foff = 0;
+        }
+      } else if (kRegistered) {
         if (foff < a.n_stacks) {
           const uint4 s0 = __ldg(a.stacks + 2 * foff), s1 = __ldg(a.stacks + 2 * foff + 1);
           k.hi = ((unsigned long long)s0.y << 32) | s0.x;
@@ -3240,6 +3261,93 @@ __global__ void __launch_bounds__(kThreads) k_lz4_pack_parts(const Lz4Blk* __res
   if (lane < 4) o[lane] = (uint8_t)(sz >> (8 * lane));
   if (sz >> 31) lz4_warp_copy(o + 4, k.src, n, lane);
   else lz4_warp_copy(o + 4, slots + (size_t)b * kLz4Block, n, lane);
+}
+
+// ---------------------------------------------------------------------------------------------
+// PA_CFG_RETIRE_STACKS: the device-resident stack registry (records, per-slot last_use words, the frame arena).
+// Record updates: upd[i] goes to slot[i]. A record with kStackFree in pad frees its slot. Any other is a registration whose
+// `off` counts from `base`, where its frames were uploaded; its last_use starts at seq[i], the batches staged before it was
+// registered, so a stack is idle for k batches only once it was registered before them.
+__global__ void __launch_bounds__(kThreads) k_stack_scatter(const RegStack* __restrict__ upd, const uint32_t* __restrict__ slot,
+                                                            const uint32_t* __restrict__ seq, uint32_t n, unsigned long long base,
+                                                            RegStack* __restrict__ recs, uint32_t* __restrict__ last_use) {
+  for (uint32_t i = blockIdx.x * kThreads + threadIdx.x; i < n; i += gridDim.x * kThreads) {
+    RegStack r = upd[i];
+    if (!(r.pad & kStackFree)) {
+      r.off += base;
+      last_use[slot[i]] = seq[i];
+    }
+    recs[slot[i]] = r;
+  }
+}
+
+// Idle selection: bit i = slot i is live and its last_use is at most `bound` (neither registered nor named in the window).
+// The bitmap goes through WordsF (exclusive popcount prefix) and k_stack_idle_emit writes the handles in slot order.
+__global__ void __launch_bounds__(kThreads) k_stack_idle_bits(const RegStack* __restrict__ recs, const uint32_t* __restrict__ last_use, uint32_t n,
+                                                              uint32_t bound, uint32_t* __restrict__ bits) {
+  const uint32_t n32 = (n + 31u) & ~31u;  // whole warps: the ballot needs every lane
+  for (uint32_t i = blockIdx.x * kThreads + threadIdx.x; i < n32; i += gridDim.x * kThreads) {
+    const bool idle = i < n && !(recs[i].pad & kStackFree) && last_use[i] <= bound;
+    const uint32_t w = __ballot_sync(0xFFFFFFFFu, idle);
+    if ((threadIdx.x & 31u) == 0) bits[i >> 5] = w;
+  }
+}
+// The first `cap` idle slots are retired: their handles go out in slot order and their last_use becomes 0xFFFFFFFF, which keeps
+// them out of every later selection while they wait for their grace batch (a row of that batch may overwrite it with a
+// sequence number that is inside every later window).
+__global__ void __launch_bounds__(kThreads) k_stack_idle_emit(const uint32_t* __restrict__ bits, const uint32_t* __restrict__ wprefix, uint32_t n,
+                                                              const RegStack* __restrict__ recs, unsigned long long cap,
+                                                              unsigned long long* __restrict__ handles, uint32_t* __restrict__ last_use) {
+  for (uint32_t i = blockIdx.x * kThreads + threadIdx.x; i < n; i += gridDim.x * kThreads) {
+    const uint32_t w = bits[i >> 5];
+    if (!((w >> (i & 31u)) & 1u)) continue;
+    const uint32_t rank = wprefix[i >> 5] + (uint32_t)__popc(w & ((1u << (i & 31u)) - 1u));
+    if (rank >= cap) continue;
+    handles[rank] = ((unsigned long long)recs[i].pad << 32) | i;
+    last_use[i] = 0xFFFFFFFFu;
+  }
+}
+
+// Arena compaction: the live stacks' frames move, in slot order, into a fresh buffer. One scan over the slots gives each live
+// stack its new offset (frames) and its copy chunks (kCompactChunk ids each), so a 65535-id stack is spread over 256 warps
+// instead of holding one.
+constexpr uint32_t kCompactChunk = 256;
+struct StackLiveF {
+  typedef Pair T;  // {chunks, frames}
+  const RegStack* recs;
+  uint32_t n_slots;
+  unsigned long long* new_off;
+  uint2* chunks;  // (slot, chunk index in the stack)
+  Pair* total_out;
+  __device__ uint32_t n() const { return n_slots; }
+  __device__ Pair value(uint32_t i) const {
+    const RegStack& r = recs[i];
+    const uint32_t d = (r.pad & kStackFree) ? 0u : r.depth;
+    return Pair{(d + kCompactChunk - 1) / kCompactChunk, d};
+  }
+  __device__ void emit(uint32_t i, Pair ex, Pair v) const {
+    new_off[i] = ex.fr;
+    for (uint32_t c = 0; c < v.cnt; c++) chunks[ex.cnt + c] = make_uint2(i, c);
+  }
+  __device__ void total(int, Pair t) const { *total_out = t; }
+};
+// one warp per chunk; `words` = 32-bit words per frame id (the arena holds the ids at the ring's width)
+__global__ void __launch_bounds__(kThreads) k_stack_compact_copy(const Pair* __restrict__ total, const uint2* __restrict__ chunks, const RegStack* __restrict__ recs,
+                                                                 const unsigned long long* __restrict__ new_off, uint32_t words,
+                                                                 const uint32_t* __restrict__ src, uint32_t* __restrict__ dst) {
+  const uint32_t lane = threadIdx.x & 31u, nc = total->cnt;
+  for (uint32_t c = (blockIdx.x * kThreads + threadIdx.x) >> 5; c < nc; c += (gridDim.x * kThreads) >> 5) {
+    const uint2 e = chunks[c];
+    const unsigned long long j0 = (unsigned long long)e.y * kCompactChunk;
+    const uint32_t cnt = min(kCompactChunk, (uint32_t)(recs[e.x].depth - j0)) * words;
+    const uint32_t* s = src + (recs[e.x].off + j0) * words;
+    uint32_t* d = dst + (new_off[e.x] + j0) * words;
+    for (uint32_t k = lane; k < cnt; k += 32) d[k] = s[k];
+  }
+}
+__global__ void __launch_bounds__(kThreads) k_stack_rebase(RegStack* __restrict__ recs, uint32_t n, const unsigned long long* __restrict__ new_off) {
+  for (uint32_t i = blockIdx.x * kThreads + threadIdx.x; i < n; i += gridDim.x * kThreads)
+    if (!(recs[i].pad & kStackFree)) recs[i].off = new_off[i];
 }
 
 }  // namespace pa

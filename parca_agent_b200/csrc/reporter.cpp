@@ -44,8 +44,19 @@ struct AggSink final : Sink {
   uint64_t RegisterStack(const TraceHash& h, const uint64_t* ids, uint32_t n) override {
     const uint64_t hash[2] = {h.hi, h.lo}, off[2] = {0, n};
     uint64_t id = ~0ull;
-    if (pa_agg_register_stacks(a, hash_mode == PA_HASH_PROVIDED ? hash : nullptr, ids, off, 1, &id) != PA_OK) return ~0ull;
+    // (the handle: the consecutive id on a plain registered aggregator, generation << 32 | slot with PA_CFG_RETIRE_STACKS)
+    if (pa_agg_register_stack_handles(a, hash_mode == PA_HASH_PROVIDED ? hash : nullptr, ids, off, 1, &id) != PA_OK) return ~0ull;
     return id;
+  }
+  int RetireStacks(uint32_t idle, std::vector<uint64_t>* handles) override {
+    std::vector<uint64_t> buf(1u << 16);
+    for (;;) {  // a call retires at most buf.size() stacks; the next one finds the rest
+      uint64_t n = 0;
+      int rc = pa_agg_retire_stacks(a, idle, buf.data(), buf.size(), &n);
+      if (rc != PA_OK) return rc;
+      handles->insert(handles->end(), buf.begin(), buf.begin() + n);
+      if (n < buf.size()) return PA_OK;
+    }
   }
   int Submit(const pa_sample_hdr& hdr, const uint64_t* frame_ids) override {
     pend_h.push_back(hdr);
@@ -117,6 +128,8 @@ void ParcaReporter::ReportExecutable(const ExecutableMetadata& md) {
     trace_ids_.clear();
     stack_cache_.clear();  // and so may registered stacks: their next sighting registers them again
     zero_hash_stacks_.clear();
+    hash_of_stack_.clear();  // (the old copies go idle and are retired; their handles are no longer in the caches)
+    zero_key_of_stack_.clear();
   }
 }
 
@@ -253,13 +266,41 @@ uint64_t ParcaReporter::stackId(const Trace* trace) {
   }
   const uint64_t id = sink_->RegisterStack(trace->Hash, scratch_ids_.data(), (uint32_t)nfr);
   if (id == ~0ull) return id;
+  const bool index = cfg_.retireIdleBatches != 0;
   if (by_hash) {
-    if (stack_cache_.size() >= kTraceCacheEntries) stack_cache_.clear();
+    if (stack_cache_.size() >= kTraceCacheEntries) { stack_cache_.clear(); hash_of_stack_.clear(); }
     stack_cache_.put(trace->Hash, id, (uint32_t)nfr);
+    if (index) hash_of_stack_[id] = trace->Hash;
   } else {
+    if (index) zero_key_of_stack_[id] = key;
     zero_hash_stacks_.emplace(std::move(key), id);
   }
   return id;
+}
+
+// Retired handles leave the caches under the ingest lock, before the next flush: a row that still names one was committed before
+// this point and lands in the next batch, which resolves it exactly (the grace batch). A cache entry that has meanwhile been
+// replaced by another handle for the same key stays.
+int ParcaReporter::retireStacks() {
+  std::vector<uint64_t> gone;
+  int rc = sink_->RetireStacks(cfg_.retireIdleBatches, &gone);
+  std::lock_guard<std::mutex> g(mu_);
+  for (uint64_t h : gone) {
+    auto k = hash_of_stack_.find(h);
+    if (k != hash_of_stack_.end()) {
+      const TraceSlot* s = stack_cache_.find(k->second);
+      if (s && s->off == h) stack_cache_.erase(k->second);
+      hash_of_stack_.erase(k);
+    }
+    auto z = zero_key_of_stack_.find(h);
+    if (z != zero_key_of_stack_.end()) {
+      auto e = zero_hash_stacks_.find(z->second);
+      if (e != zero_hash_stacks_.end() && e->second == h) zero_hash_stacks_.erase(e);
+      zero_key_of_stack_.erase(z);
+    }
+  }
+  stacksRetired += gone.size();
+  return rc;
 }
 
 int ParcaReporter::ReportTraceEvent(const Trace* trace, const TraceEventMeta* meta) {
@@ -375,6 +416,7 @@ int64_t ParcaReporter::FlushOnce() {
   }
   const uint64_t n_unique = res.n_unique_stacks;
   sink_->Release(&res);
+  if (cfg_.registeredStacks && cfg_.retireIdleBatches) retireStacks();  // (a failed call is retried after the next flush)
   if (rows && cfg_.offlineV1Stacktraces) {
     // :1300-1349 — walk the sample record's stacktrace_id dictionary in order, keep the ids this log has not
     // seen, and write their stacktrace record right behind the sample record (even when there are none)

@@ -89,6 +89,9 @@ struct Sink {
   virtual int Submit(const pa_sample_hdr& hdr, const uint64_t* frame_ids) = 0;  // may buffer rows until Publish
   // Config::registeredStacks: register one stack (its trace hash and frame ids); returns its stack id, ~0 on failure
   virtual uint64_t RegisterStack(const TraceHash& /*hash*/, const uint64_t* /*ids*/, uint32_t /*n*/) { return ~0ull; }
+  // Config::retireIdleBatches (PA_CFG_RETIRE_STACKS aggregator): retire the stacks no batch has named for `idle` batches and
+  // append their handles to *handles; called after a flush, on the flushing thread. Returns 0 or a PA_E* code.
+  virtual int RetireStacks(uint32_t /*idle*/, std::vector<uint64_t>* /*handles*/) { return PA_EINVAL; }
   virtual int Publish() { return 0; }  // hand buffered rows to the aggregator; called under the reporter's ingest lock
   virtual int Flush(pa_agg_result* out) = 0;
   virtual void Release(pa_agg_result* res) = 0;
@@ -99,6 +102,60 @@ struct Sink {
 // owns nothing; forwards to the C ABI. hash_mode: the aggregator's (RegisterStack passes the trace hash in PA_HASH_PROVIDED mode
 // only; in PA_HASH_XXH64X2 mode the library computes the stack id)
 Sink* NewAggSink(pa_agg* agg, uint32_t hash_mode = PA_HASH_PROVIDED);
+
+// trace.Hash -> (off, n): open addressing with linear probing in one flat array (a hit is one cache line, where a node-based map
+// takes a bucket and a node). erase() shifts the rest of the probe chain back, so no tombstones are left behind.
+struct TraceSlot { TraceHash key; uint64_t off; uint32_t n; uint32_t used; };
+struct TraceCache {
+  std::vector<TraceSlot> slots;
+  size_t count = 0;
+  static size_t home(const TraceHash& h, size_t mask) { return (size_t)(h.hi * 0x9E3779B97F4A7C15ull ^ h.lo) & mask; }
+  const TraceSlot* find(const TraceHash& h) const {
+    if (slots.empty()) return nullptr;
+    const size_t mask = slots.size() - 1;
+    for (size_t i = home(h, mask);; i = (i + 1) & mask) {
+      const TraceSlot& s = slots[i];
+      if (!s.used) return nullptr;
+      if (s.key.hi == h.hi && s.key.lo == h.lo) return &s;
+    }
+  }
+  void put(const TraceHash& h, uint64_t off, uint32_t n) {
+    if (slots.empty()) slots.resize(1u << 16);
+    if ((count + 1) * 4 > slots.size() * 3) {  // grow (rehash); the reporter clears the cache at kTraceCacheEntries
+      std::vector<TraceSlot> old;
+      old.swap(slots);
+      slots.resize(old.size() * 2);
+      count = 0;
+      for (auto& s : old) if (s.used) put(s.key, s.off, s.n);
+    }
+    const size_t mask = slots.size() - 1;
+    for (size_t i = home(h, mask);; i = (i + 1) & mask) {
+      TraceSlot& s = slots[i];
+      if (!s.used) { s = TraceSlot{h, off, n, 1u}; count++; return; }
+      if (s.key.hi == h.hi && s.key.lo == h.lo) { s.off = off; s.n = n; return; }
+    }
+  }
+  // backward-shift deletion: every later entry of the chain whose home is not in (hole, entry] moves into the hole
+  bool erase(const TraceHash& h) {
+    if (slots.empty()) return false;
+    const size_t mask = slots.size() - 1;
+    size_t i = home(h, mask);
+    for (;; i = (i + 1) & mask) {
+      if (!slots[i].used) return false;
+      if (slots[i].key.hi == h.hi && slots[i].key.lo == h.lo) break;
+    }
+    for (size_t j = (i + 1) & mask; slots[j].used; j = (j + 1) & mask) {
+      const size_t k = home(slots[j].key, mask);
+      const bool stays = i <= j ? (i < k && k <= j) : (i < k || k <= j);
+      if (!stays) { slots[i] = slots[j]; i = j; }
+    }
+    slots[i].used = 0;
+    count--;
+    return true;
+  }
+  void clear() { slots.clear(); count = 0; }
+  size_t size() const { return count; }
+};
 
 struct Config {
   std::string nodeName;
@@ -117,6 +174,9 @@ struct Config {
   // Sink::RegisterStack and its rows carry the stack id in frame_off with no frame ids. Traces are keyed by trace.Hash, the
   // zero hash (oomprof traces) by the frame-id list.
   bool registeredStacks = false;
+  // with registeredStacks, on a PA_CFG_RETIRE_STACKS aggregator: after every flush, retire the stacks no batch has named for this
+  // many batches (Sink::RetireStacks) and forget their handles, so their traces register again on their next sighting. 0 = off.
+  uint32_t retireIdleBatches = 0;
 };
 
 class ParcaReporter {
@@ -145,7 +205,7 @@ class ParcaReporter {
 
   // counters mirroring :899-941
   std::atomic<uint64_t> cpuSamples{0}, offcpuSamples{0}, memorySamples{0}, gpuSamples{0}, emptySamples{0}, skippedByRelabeling{0},
-      sampleWrites{0}, sampleWriteRequestBytes{0}, droppedBatches{0}, stacktraceWriteRequestBytes{0};
+      sampleWrites{0}, sampleWriteRequestBytes{0}, droppedBatches{0}, stacktraceWriteRequestBytes{0}, stacksRetired{0};
 
  private:
   struct PidLabels { uint32_t labelset = 0; bool keep = true; Labels base; };
@@ -163,45 +223,17 @@ class ParcaReporter {
   // cleared when full and whenever an executable becomes known (frames resolved as UNKNOWN must be looked at again).
   struct TraceHashHasher { size_t operator()(const TraceHash& h) const { return (size_t)(h.hi * 0x9E3779B97F4A7C15ull ^ h.lo); } };
   struct TraceHashEq { bool operator()(const TraceHash& a, const TraceHash& b) const { return a.hi == b.hi && a.lo == b.lo; } };
-  // trace.Hash -> (offset, count) in trace_ids_: open addressing in one flat array (a hit is one cache line, where a node-based map
-  // takes a bucket and a node), cleared as a whole when it is three quarters full
-  struct TraceSlot { TraceHash key; uint64_t off; uint32_t n; uint32_t used; };
-  struct TraceCache {
-    std::vector<TraceSlot> slots;
-    size_t count = 0;
-    const TraceSlot* find(const TraceHash& h) const {
-      if (slots.empty()) return nullptr;
-      const size_t mask = slots.size() - 1;
-      for (size_t i = (size_t)(h.hi * 0x9E3779B97F4A7C15ull ^ h.lo) & mask;; i = (i + 1) & mask) {
-        const TraceSlot& s = slots[i];
-        if (!s.used) return nullptr;
-        if (s.key.hi == h.hi && s.key.lo == h.lo) return &s;
-      }
-    }
-    void put(const TraceHash& h, uint64_t off, uint32_t n) {
-      if (slots.empty()) slots.resize(1u << 16);
-      if ((count + 1) * 4 > slots.size() * 3) {  // grow (rehash) up to kTraceCacheEntries slots; beyond that the caller clears
-        std::vector<TraceSlot> old;
-        old.swap(slots);
-        slots.resize(old.size() * 2);
-        count = 0;
-        for (auto& s : old) if (s.used) put(s.key, s.off, s.n);
-      }
-      const size_t mask = slots.size() - 1;
-      for (size_t i = (size_t)(h.hi * 0x9E3779B97F4A7C15ull ^ h.lo) & mask;; i = (i + 1) & mask) {
-        TraceSlot& s = slots[i];
-        if (!s.used) { s = TraceSlot{h, off, n, 1u}; count++; return; }
-        if (s.key.hi == h.hi && s.key.lo == h.lo) { s.off = off; s.n = n; return; }
-      }
-    }
-    void clear() { slots.clear(); count = 0; }
-    size_t size() const { return count; }
-  } trace_cache_;
+  // trace.Hash -> (offset, count) in trace_ids_, cleared as a whole when it is three quarters full
+  TraceCache trace_cache_;
   std::vector<uint64_t> trace_ids_;
   std::vector<uint64_t> scratch_ids_;
   // Config::registeredStacks: trace.Hash -> stack id (off = the id, n = the depth), and frame-id list -> stack id for the zero hash
   TraceCache stack_cache_;
   std::unordered_map<std::string, uint64_t> zero_hash_stacks_;
+  // Config::retireIdleBatches: stack handle -> its key in stack_cache_ / zero_hash_stacks_ (cleared with them), so the handles a
+  // retirement returns can be dropped from the caches
+  std::unordered_map<uint64_t, TraceHash> hash_of_stack_;
+  std::unordered_map<uint64_t, std::string> zero_key_of_stack_;
   static constexpr size_t kTraceCacheEntries = 1u << 20;
   std::map<FileID, ExecutableMetadata> executables_;          // r.executables (:650-693)
   std::map<FileID, std::vector<std::string>> unknown_by_file_;  // frames interned while their executable was unknown
@@ -219,6 +251,7 @@ class ParcaReporter {
   bool labelsForPID(uint32_t pid, PidLabels** out);
   int writeSampleV2(const Trace* trace, const TraceEventMeta* meta, uint32_t labelset, uint8_t kind, int64_t value, const uint64_t* ids, size_t nids);
   uint64_t stackId(const Trace* trace);  // Config::registeredStacks: the trace's stack id, registered on first sight; ~0 = failed
+  int retireStacks();                    // Config::retireIdleBatches: after a flush
 };
 
 // maybeFixTruncation (parca_reporter.go:190-216)

@@ -21,7 +21,7 @@ EXPORTS = [
     "pa_agg_debug_stack_ids", "pa_agg_debug_stack_counts", "pa_agg_debug_pair_counts", "pa_agg_stacktraces", "pa_agg_last_stack_ids", "pa_agg_shard_sizes", "pa_agg_shard_export", "pa_agg_stage_device", "pa_agg_stage_device_parts", "pa_agg_discard", "pa_ipc_compress_lz4", "pa_ipc_free", "pa_fix_truncation", "pa_xxh64",
     "pa_merge_create_local", "pa_merge_nccl_unique_id", "pa_merge_create_nccl", "pa_merge_destroy", "pa_merge_last_error", "pa_merge_process",
     "pa_merge_plan", "pa_merge_collect", "pa_merge_flush", "pa_merge_last_stats", "pa_merge_create_host", "pa_merge_create_shm",
-    "pa_merge_stacktraces",
+    "pa_merge_stacktraces", "pa_agg_register_stack_handles", "pa_agg_retire_stacks",
 ]
 
 
@@ -49,6 +49,8 @@ def lib():
         L.pa_agg_register_frames.argtypes = [vp, vp, C.c_uint32, u64p]
         L.pa_agg_register_labelsets.argtypes = [vp, vp, vp, C.c_uint32, u32p]
         L.pa_agg_register_stacks.argtypes = [vp, vp, vp, vp, C.c_uint32, u64p]
+        L.pa_agg_register_stack_handles.argtypes = [vp, vp, vp, vp, C.c_uint32, vp]
+        L.pa_agg_retire_stacks.argtypes = [vp, C.c_uint32, vp, C.c_uint64, u64p]
         L.pa_agg_acquire.argtypes = [vp, C.c_uint64, C.c_uint64, C.POINTER(vp), C.POINTER(vp), u64p]
         L.pa_agg_commit.argtypes = [vp, C.c_uint64]
         L.pa_agg_submit.argtypes = [vp, vp, vp, C.c_uint64]
@@ -184,6 +186,32 @@ class Aggregator:
         self._ck(lib().pa_agg_register_stacks(self.h, None if hashes is None else hashes.ctypes.data, frames.ctypes.data if len(frames) else None,
                                               offsets.ctypes.data, n, C.byref(first)))
         return first.value
+
+    def register_stack_handles(self, frames, offsets, hashes=None):
+        """register_stacks for either registered mode: a uint64 array with the handle of each stack (PA_CFG_RETIRE_STACKS:
+        generation << 32 | slot; otherwise the consecutive ids)."""
+        frames = np.ascontiguousarray(frames, dtype=self.id_dtype)
+        offsets = np.ascontiguousarray(offsets, dtype=np.uint64)
+        n = len(offsets) - 1
+        if hashes is not None:
+            hashes = np.ascontiguousarray(hashes, dtype=np.uint64).reshape(-1)
+        out = np.zeros(max(n, 1), dtype=np.uint64)
+        self._ck(lib().pa_agg_register_stack_handles(self.h, None if hashes is None else hashes.ctypes.data, frames.ctypes.data if len(frames) else None,
+                                                     offsets.ctypes.data, n, out.ctypes.data))
+        return out[:n]
+
+    def retire_stacks(self, idle_batches, cap=None):
+        """PA_CFG_RETIRE_STACKS: retire the stacks idle for `idle_batches` batches (at most `cap`, default all); returns their
+        handles in slot order. Drop them from any lookup before the next flush."""
+        cap = self.stack_counters()["stacks_live"] if cap is None else cap
+        out = np.zeros(max(cap, 1), dtype=np.uint64)
+        n = C.c_uint64()
+        self._ck(lib().pa_agg_retire_stacks(self.h, idle_batches, out.ctypes.data, cap, C.byref(n)))
+        return out[:n.value]
+
+    def stack_counters(self):
+        """PA_CFG_RETIRE_STACKS: the stack registry's counters (pa_agg_last_kernel_ms names)."""
+        return {k: self.kernel_ms(k)[1] for k in ("stacks_live", "stacks_free", "stack_frames_live", "stack_frames_dead", "stack_compactions", "stacks_retired")}
 
     # ---- ingest
     def submit(self, hdrs, frame_ids):
@@ -508,7 +536,7 @@ def from_workload(w, device=0, max_samples=None, max_frames=None, chunk_samples=
     a.register_labelsets(w.labelsets)
     if sf is not None:
         a.stack_form = sf
-        a.register_stacks(sf.frames, sf.offsets, sf.hashes if w.hash_mode == abi.PA_HASH_PROVIDED else None)
+        a.register_stack_handles(sf.frames, sf.offsets, sf.hashes if w.hash_mode == abi.PA_HASH_PROVIDED else None)
     return a
 
 
