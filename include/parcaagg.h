@@ -111,6 +111,17 @@ enum {
                                     freed (live, pending, and retired ones still in their grace batch); the frames freed stacks leave
                                     behind do not count, and the device arena is compacted when they outweigh the live ones. The
                                     output is byte for byte the same as without the flag */
+#define PA_CFG_GROUP_RETIRE 0x10u /* only as PA_CFG_REGISTERED_STACKS | PA_CFG_GROUP_STACKS | PA_CFG_GROUP_RETIRE (pa_agg_create fails with
+                                    PA_EINVAL otherwise, and with PA_CFG_RETIRE_STACKS): retirement for the members of a merge group.
+                                    Stacks are named by handles and registered through pa_agg_register_stack_handles, as with
+                                    PA_CFG_RETIRE_STACKS, but the group retires them, collectively (pa_merge_retire_stacks): a stack that
+                                    any member's rows named in the idle window stays live, and every member's slots, generations and free
+                                    slots stay identical, so identical registrations return identical handles on every member.
+                                    pa_agg_retire_stacks is refused (PA_EINVAL); the registry counters of PA_CFG_RETIRE_STACKS work.
+                                    pa_merge_process checks the members' slot count, stage count and a digest of every registration
+                                    (handle, id, depth, frame ids) and retirement, and fails with PA_EINVAL on every rank when they
+                                    differ: a member staged or flushed on its own has left the group's lockstep. A group cannot mix such
+                                    members with other members (refused like a mixed PA_CFG_GROUP_STACKS group) */
 
 #define PA_NO_STRING 0xFFFFFFFFu /* "no value"; string id 0 is always the empty string "" */
 
@@ -403,6 +414,17 @@ int pa_merge_plan(pa_merge* m, uint64_t* ipc_len);
 int pa_merge_collect(pa_merge* m, uint8_t* base, uint64_t cap, pa_agg_result* out);
 /* in-process groups: ring swap + H2D of every member, the merged pass, plan and collect in one call */
 int pa_merge_flush(pa_merge* m, pa_agg_result* out);
+/* PA_CFG_GROUP_RETIRE groups, between intervals (collective: every rank calls it after pa_merge_collect, with the same arguments).
+ * pa_agg_retire_stacks for the whole group, with the same rules (idle window, cap, lowest slot first, grace batch): a stack is idle
+ * when no member's rows named it in the window. Every rank receives the same handles in handles[] (ascending slot order) and
+ * *n_retired, and every member frees the same slots at the same stage. PA_EINVAL on every rank, with nothing retired, for
+ * idle_batches == 0, a member whose staged batch is not collected, a member without the flag, and ranks that disagree on
+ * idle_batches, cap, stage count or uploaded slot count. handles[] receives at most min(cap, uploaded slots) entries, so a caller
+ * that wants every idle stack may pass cap = UINT64_MAX (the same on every rank) with room for its member's slots. Registrations
+ * may run concurrently on any member (the registry digest keeps registrations and retirements apart, so their interleaving on
+ * each member does not matter). The caller drops the returned handles from its lookup before the next interval's rows are
+ * written. */
+int pa_merge_retire_stacks(pa_merge* m, uint32_t idle_batches, uint64_t* handles, uint64_t cap, uint64_t* n_retired);
 /* v1 groups, between intervals (collective): the stacktrace record (pa_agg_stacktraces) for rank 0's request. Rank 0 passes the
  * server's ids, the other ranks NULL / 0 (the ids reach them in one all-gather). Every member applies the request's accesses to
  * its copy of the store, and each rank's *out is the record its own member built: the same bytes on every rank (in-process

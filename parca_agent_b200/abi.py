@@ -12,6 +12,7 @@ PA_CFG_SINGLE_RING = 1
 PA_CFG_REGISTERED_STACKS = 2
 PA_CFG_GROUP_STACKS = 4
 PA_CFG_RETIRE_STACKS = 8
+PA_CFG_GROUP_RETIRE = 16
 
 PA_KIND_CPU, PA_KIND_OFFCPU, PA_KIND_CUDA = 0, 1, 2
 PA_KIND_MEM_INUSE_OBJECTS, PA_KIND_MEM_INUSE_SPACE, PA_KIND_MEM_ALLOC_OBJECTS, PA_KIND_MEM_ALLOC_SPACE = 3, 4, 5, 6

@@ -109,6 +109,7 @@ struct Pass {
   uint32_t n_stacks = 0;          // registered stacks (PA_CFG_REGISTERED_STACKS)
   uint64_t n_stack_frames = 0;    // and the frame ids of their arena
   uint64_t stack_digest = 0;      // PA_CFG_GROUP_STACKS: digest of those stacks (merge groups check it is the same on every member)
+  uint64_t stack_frames_live = 0; // PA_CFG_GROUP_RETIRE: frames of the uploaded stacks not yet freed (the same on every member)
   uint64_t N = 0, NT = 0, row_base = 0;
   uint32_t world = 1, rank = 0, ncols = 0, nlab = 0;
   bool v1 = false, provided = false, merged = false;  // provided: the stack ids arrive with the rows (or their registered stacks)
@@ -187,7 +188,12 @@ struct pa_agg {
   // PA_CFG_REGISTERED_STACKS: the registered stacks and their frame arena (ids at the ring's width, idb / 4 words each)
   bool registered = false;
   bool group_stacks = false;  // PA_CFG_GROUP_STACKS: the stack ids are group-wide (merge groups)
-  uint64_t reg_digest = 0;    // PA_CFG_GROUP_STACKS: running digest of every registered stack's (id, depth, frame ids)
+  uint64_t reg_digest = 0;    // PA_CFG_GROUP_STACKS: running digest of every registered stack's (id, depth, frame ids); with
+                              // PA_CFG_GROUP_RETIRE of (handle, id, depth, frame ids)
+  // PA_CFG_GROUP_RETIRE: running digest of every group retirement's (idle_batches, handles), kept apart from reg_digest so that a
+  // registration running concurrently with pa_merge_retire_stacks may land before or after it on each member; rs_upload combines
+  // the two
+  uint64_t retire_digest = 0;
   std::vector<RegStack> reg_stacks;
   std::vector<uint32_t> reg_arena;
   Mirror<RegStack> m_stacks;
@@ -196,6 +202,7 @@ struct pa_agg {
   // the free slots (a min-heap), the retired stacks waiting for their grace batch, and the registrations not yet uploaded.
   enum : uint8_t { RS_LIVE, RS_RETIRING, RS_FREE };
   bool retire = false;
+  bool group_retire = false;  // PA_CFG_GROUP_RETIRE (retire is set too): the merge group retires, through pa_merge_retire_stacks
   std::vector<uint32_t> rs_depth, rs_gen;  // rs_gen: the generation of the slot's current (or next) stack
   std::vector<uint8_t> rs_state;
   std::vector<uint32_t> rs_free;
@@ -408,6 +415,8 @@ int pa_agg_create(const pa_agg_config* cfg, pa_agg** out) {
       (cfg->frame_id_bytes != 0 && cfg->frame_id_bytes != 4 && cfg->frame_id_bytes != 8)) return PA_EINVAL;
   if ((cfg->flags & PA_CFG_GROUP_STACKS) && !(cfg->flags & PA_CFG_REGISTERED_STACKS)) return PA_EINVAL;
   if ((cfg->flags & PA_CFG_RETIRE_STACKS) && (!(cfg->flags & PA_CFG_REGISTERED_STACKS) || (cfg->flags & PA_CFG_GROUP_STACKS))) return PA_EINVAL;
+  if ((cfg->flags & PA_CFG_GROUP_RETIRE) &&
+      ((cfg->flags & PA_CFG_RETIRE_STACKS) || !(cfg->flags & PA_CFG_REGISTERED_STACKS) || !(cfg->flags & PA_CFG_GROUP_STACKS))) return PA_EINVAL;
   if (cfg->max_samples > 0x7FFFFFFFull) return PA_ERANGE;  // run ends / ListView offsets are int32
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || cfg->device < 0 || cfg->device >= ndev) return PA_ENODEV;
@@ -420,7 +429,8 @@ int pa_agg_create(const pa_agg_config* cfg, pa_agg** out) {
   a->single_ring = (cfg->flags & PA_CFG_SINGLE_RING) != 0;
   a->registered = (cfg->flags & PA_CFG_REGISTERED_STACKS) != 0;
   a->group_stacks = (cfg->flags & PA_CFG_GROUP_STACKS) != 0;
-  a->retire = (cfg->flags & PA_CFG_RETIRE_STACKS) != 0;
+  a->group_retire = (cfg->flags & PA_CFG_GROUP_RETIRE) != 0;
+  a->retire = (cfg->flags & PA_CFG_RETIRE_STACKS) != 0 || a->group_retire;
   auto bail = [&](int code) { pa_agg_destroy(a); return code; };
   if (cudaSetDevice(a->device) != cudaSuccess) return bail(PA_ENODEV);
   cudaDeviceProp prop;
@@ -733,6 +743,12 @@ int pa_agg_register_stack_handles(pa_agg* a, const uint64_t* hashes, const uint6
     a->rs_state[slot] = pa_agg::RS_LIVE; a->rs_depth[slot] = (uint32_t)d;
     a->rs_live++; a->rs_frames_live += d;
     handles[i] = ((uint64_t)a->rs_gen[slot] << 32) | slot;
+    if (a->group_retire) {  // the registry's digest, as for PA_CFG_GROUP_STACKS with the handle in front
+      wide.resize(d + 4);
+      wide[0] = handles[i]; wide[1] = s.hash_hi; wide[2] = s.hash_lo; wide[3] = d;
+      for (uint64_t j = 0; j < d; j++) wide[4 + j] = a->idb == 4 ? (uint64_t)((const uint32_t*)frames)[offsets[i] + j] : frames[offsets[i] + j];
+      a->reg_digest = pa_xxh64(wide.data(), (d + 4) * 8, a->reg_digest);
+    }
   }
   return PA_OK;
 }
@@ -976,6 +992,9 @@ static int rs_upload(pa_agg* a, const std::vector<RegStack>& frees, const std::v
   a->src_frames = (const unsigned long long*)a->d_rs_arena[a->rs_cur].p;
   a->P.n_stacks = (uint32_t)n_slots;
   a->P.n_stack_frames = a->rs_dev_len;
+  const uint64_t digests[2] = {a->reg_digest, a->retire_digest};
+  a->P.stack_digest = pa_xxh64(digests, sizeof digests, 0);
+  a->P.stack_frames_live = a->rs_frames_live;  // (nothing is pending now: these are the uploaded stacks not yet freed)
   return PA_OK;
 }
 
@@ -2875,6 +2894,7 @@ extern "C" {
 
 int pa_agg_retire_stacks(pa_agg* a, uint32_t idle_batches, uint64_t* handles, uint64_t cap, uint64_t* n_retired) {
   if (!a) return PA_EINVAL;
+  if (a->group_retire) return a->fail(PA_EINVAL, "PA_CFG_GROUP_RETIRE: the merge group retires its stacks together, through pa_merge_retire_stacks");
   std::lock_guard<std::mutex> g(a->flush_mu);
   return retire_stacks(a, idle_batches, handles, cap, n_retired);
 }

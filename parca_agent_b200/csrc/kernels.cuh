@@ -2375,6 +2375,10 @@ struct StoreInsertArgs {
   // k_store_insert<true, true> (PA_CFG_GROUP_STACKS): g_foff indexes g_refs instead, one entry per stack; the frames are read from
   // this member's own registered arena (`frames`), which is the same on every member
   const unsigned long long* g_refs;  // arena offset of each needed stack's frames, from its global first occurrence
+  // k_store_insert<true, true, true> (PA_CFG_GROUP_RETIRE): g_refs holds handles, resolved through this member's own records, since
+  // the members' arenas may be laid out differently (compactions at different points of the registrations)
+  const uint4* g_recs;               // RegStack records, two uint4 each
+  uint32_t n_recs;
 };
 // last occurrence of every stack of the batch (the LRU's access time of its entry)
 __global__ void __launch_bounds__(kThreads) k_last_rows(uint32_t n_rows, const uint32_t* slot_of_row, uint32_t* last_row) {
@@ -2418,7 +2422,8 @@ __global__ void __launch_bounds__(kThreads) k_store_kill(unsigned long long* sta
 // one warp per unique stack of the batch (unique within the launch, so a key is claimed by at most one warp).
 // MERGED: one replica of a merge group's store; u is the merged ordinal, frames come from the gathered buffer.
 // REFS (with MERGED): frames come from the member's registered arena, at the gathered offset (g_refs).
-template <bool MERGED, bool REFS = false>
+// HANDLES (with REFS): g_refs holds each stack's handle instead; the member's own record (g_recs) gives the offset.
+template <bool MERGED, bool REFS = false, bool HANDLES = false>
 __global__ void __launch_bounds__(kThreads) k_store_insert(StoreInsertArgs a) {
   const unsigned full = 0xFFFFFFFFu;
   uint32_t nu = a.ctr->n_unique;
@@ -2487,7 +2492,18 @@ __global__ void __launch_bounds__(kThreads) k_store_insert(StoreInsertArgs a) {
         if (lane == 0) atomicOr(&a.ctr_w->err, ERR_MERGE_LOOKUP);
         continue;
       }
-      const unsigned long long base = size ? a.g_refs[k] : 0ull;
+      unsigned long long base = size ? a.g_refs[k] : 0ull;
+      if constexpr (HANDLES) {
+        if (size) {  // the sender's k_header accepted this handle in this batch, so a mismatch here is a logic error
+          const uint32_t slot = (uint32_t)base, gen = (uint32_t)(base >> 32);
+          const uint4 s1 = slot < a.n_recs ? __ldg(a.g_recs + 2ull * slot + 1) : make_uint4(0u, 0u, 0u, kStackFree);
+          if (s1.w != gen || (gen & kStackFree) || s1.z != size) {
+            if (lane == 0) atomicOr(&a.ctr_w->err, ERR_MERGE_LOOKUP);
+            continue;
+          }
+          base = ((unsigned long long)s1.y << 32) | s1.x;
+        }
+      }
       for (uint32_t j = lane; j < size; j += 32) {
         unsigned long long fid = frame_at(a.frames, base + j, a.narrow);
         if (fid >= a.n_frames_registered) { atomicOr(&a.ctr_w->err, ERR_BAD_FRAME_ID); fid = 0; }
@@ -2943,6 +2959,10 @@ __global__ void __launch_bounds__(kThreads) k_tid_insert(const unsigned long lon
 __global__ void __launch_bounds__(kThreads) k_min_u32(uint32_t* dst, const uint32_t* src, size_t n) {
   for (size_t i = (size_t)blockIdx.x * kThreads + threadIdx.x; i < n; i += (size_t)gridDim.x * kThreads) { uint32_t v = src[i]; if (v < dst[i]) dst[i] = v; }
 }
+// x -> ~x in place: around an all-reduce(min), it makes a max-reduction (PA_CFG_GROUP_RETIRE: the group's last_use of each slot)
+__global__ void __launch_bounds__(kThreads) k_invert_u32(uint32_t* p, size_t n) {
+  for (size_t i = (size_t)blockIdx.x * kThreads + threadIdx.x; i < n; i += (size_t)gridDim.x * kThreads) p[i] = ~p[i];
+}
 // run-end columns across shards. edges[m][c] come from every shard (all-gather); a shard's last run continues in the next
 // non-empty shard when both border rows are non-null and carry the same key (BinaryDictionaryRunEndBuilder.Append,
 // reporter/arrow.go:97-131: a row extends the current run iff the previous value is non-null and byte-equal). The
@@ -3072,13 +3092,16 @@ struct StoreRefsF {  // where each merged stack's reference goes in the gathered
   __device__ void emit(uint32_t u, unsigned long long ex, unsigned long long) const { ridx[u] = ex; }
   __device__ void total(int, unsigned long long t) const { ridx[ctr->n_unique] = t; }
 };
-// this shard's block: the references of its won stacks that k_store_need selected
+// this shard's block: the references of its won stacks that k_store_need selected. A row's reference is ref[row * ref_stride]:
+// its frame_off after k_header (stride 1), or, in PA_CFG_GROUP_RETIRE groups, the handle its header still carries (the
+// pa_sample_hdr's frame_off word, stride 8)
 __global__ void __launch_bounds__(kThreads) k_store_pack_refs(const MergeCtl* mc, const uint32_t* g_row, uint32_t row_base, const uint32_t* need,
-                                                              const unsigned long long* ridx, const unsigned long long* frame_off, unsigned long long* out) {
+                                                              const unsigned long long* ridx, const unsigned long long* ref, uint32_t ref_stride,
+                                                              unsigned long long* out) {
   const uint32_t o0 = mc->ord0, o1 = mc->ord1;
   const unsigned long long base0 = ridx[o0];
   for (uint32_t u = o0 + blockIdx.x * kThreads + threadIdx.x; u < o1; u += gridDim.x * kThreads)
-    if (need[u]) out[ridx[u] - base0] = frame_off[g_row[u] - row_base];
+    if (need[u]) out[ridx[u] - base0] = ref[(size_t)(g_row[u] - row_base) * ref_stride];
 }
 
 // ---------------------------------------------------------------------------------------------

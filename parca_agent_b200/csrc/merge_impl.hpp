@@ -13,6 +13,9 @@
 //   v1 groups (replicated known-stacks store): all-reduce(min) of each merged stack's inverted last row  U x 4 B
 //                and all-gather-v of the frames of the stacks the store lacks                          4 B per frame (0 in steady state)
 //                (PA_CFG_GROUP_STACKS members: of one arena offset per such stack instead)             8 B per stack
+//                (PA_CFG_GROUP_RETIRE members: of the stack's handle instead)                          8 B per stack
+//   PA_CFG_GROUP_RETIRE groups, in pa_merge_retire_stacks: all-gather of the call's arguments and state   32 B
+//                and all-reduce(min) of the inverted last_use of every registry slot                   4 B per slot
 // Invariants reproduced: first-occurrence order of every dictionary (arrow_v2.go:191, :302; parca_reporter.go:425),
 // run merging across shard borders (arrow.go:97-131).
 //
@@ -153,6 +156,7 @@ struct pa_merge {
   bool lz4 = false;
   // ---- PA_CFG_GROUP_STACKS groups (every member in that mode): rows name stacks of identical registries, no ring frames
   bool group_stacks = false;
+  bool group_retire = false;  // PA_CFG_GROUP_RETIRE groups (every member in that mode): stacks are retired by the group
   struct Lz4Share {                             // one local member's blocks, from pa_merge_plan to pa_merge_collect
     Lz4Table t;
     Lz4Dev d;
@@ -194,6 +198,12 @@ static const char kStacksMixed[] = "a merge group of PA_CFG_GROUP_STACKS members
                                    "with ring members or with plain PA_CFG_REGISTERED_STACKS members";
 static const char kStacksMismatch[] = "the members of a PA_CFG_GROUP_STACKS merge group must register identical stacks in the same order: "
                                       "their number of stacks, frame arena length or stack digest differ";
+// PA_CFG_GROUP_RETIRE members retire together: a group of them takes no other members, and they stay in lockstep
+static const char kRetireMixed[] = "a merge group of PA_CFG_GROUP_RETIRE members takes no other members: this group mixes PA_CFG_GROUP_RETIRE members "
+                                   "with members that do not retire stacks as a group";
+static const char kRetireMismatch[] = "the members of a PA_CFG_GROUP_RETIRE merge group must register identical stacks in the same order, and stage "
+                                      "and retire only as a group: their slot count, live stack frames, stage count or registry digest differ "
+                                      "(a member staged or flushed on its own has left the group)";
 // Every member of a group uses the same schema; v1 members also need the same store size, since each holds a full copy of the
 // group's store (refused like a mixed LZ4 mode).
 static const char kSchemaMixed[] = "a merge group builds one record schema: this group mixes PA_SCHEMA_V1 and PA_SCHEMA_V2 members";
@@ -613,6 +623,14 @@ static int merge_process_once(pa_merge* g, bool* retry) {
   for (uint32_t r = 0; r < W; r++)
     if (hc[(size_t)r * cw + W + 1] & ERR_TABLE_FULL) { *retry = true; }
   if (*retry) return PA_OK;  // some shard's local table was too small: every member redoes the batch with larger ones
+  if (g->group_retire) {  // a stale handle is seen only by the shard whose rows carry it: every rank stops here, before the exchange
+    uint32_t e = 0;
+    for (uint32_t r = 0; r < W; r++) e |= hc[(size_t)r * cw + W + 1];
+    if (e & ERR_BAD_STACK_ID) {
+      for (size_t i = 0; i < L; i++) g->members[i]->h_ctr.err = e;
+      return PA_OK;
+    }
+  }
   // ---- pack by owner, all-to-all
   std::vector<const void*> sendp(L);
   std::vector<void*> recvp(L);
@@ -859,9 +877,12 @@ static int store_frames_exchange(pa_merge* g, uint32_t min_last_p1) {
     MCK(mb.v1_send.ensure(std::max<uint64_t>(count[me], 256)));
     MCK(mb.v1_frames.ensure(std::max<uint64_t>(b[W] * unit, 256)));
     if (refs) {
+      // group retire: the handle (the header's frame_off word), since the members' arenas may differ in layout
+      const unsigned long long* ref = g->group_retire ? a->d_hdr.as<unsigned long long>() + offsetof(pa_sample_hdr, frame_off) / 8 : a->d_foff.as<unsigned long long>();
       k_store_pack_refs<<<small_grid(a, U), kThreads, 0, a->s_comp>>>((const MergeCtl*)(mb.ctl.as<uint32_t>() + CTL_MERGE), mb.g_uniq_row.as<uint32_t>(),
                                                                       (uint32_t)g->row_base[me], mb.v1_need.as<uint32_t>(), mb.v1_foff.as<unsigned long long>(),
-                                                                      a->d_foff.as<unsigned long long>(), mb.v1_send.as<unsigned long long>());
+                                                                      ref, g->group_retire ? (uint32_t)(sizeof(pa_sample_hdr) / 8) : 1u,
+                                                                      mb.v1_send.as<unsigned long long>());
       a->store_refs_sent += count[me] / 8;
       src[i] = mb.v1_send.p; dst[i] = mb.v1_frames.p;
       continue;
@@ -929,7 +950,10 @@ static int merge_store_update(pa_merge* g) {
       StoreInsertArgs sa = store_insert_args(a, min_last_p1);
       sa.gtab = mb.gtab.as<StackSlot>(); sa.g_slot = mb.g_uniq_slot.as<uint32_t>(); sa.g_last_inv = last[i];
       sa.g_frames = mb.v1_frames.as<uint32_t>(); sa.g_foff = mb.v1_foff.as<unsigned long long>();
-      if (g->group_stacks) { sa.g_refs = mb.v1_frames.as<unsigned long long>(); k_store_insert<true, true><<<a->G, kThreads, 0, a->s_comp>>>(sa); }
+      if (g->group_retire) {
+        sa.g_refs = mb.v1_frames.as<unsigned long long>(); sa.g_recs = (const uint4*)a->d_rs_recs.p; sa.n_recs = a->P.n_stacks;
+        k_store_insert<true, true, true><<<a->G, kThreads, 0, a->s_comp>>>(sa);
+      } else if (g->group_stacks) { sa.g_refs = mb.v1_frames.as<unsigned long long>(); k_store_insert<true, true><<<a->G, kThreads, 0, a->s_comp>>>(sa); }
       else k_store_insert<true><<<a->G, kThreads, 0, a->s_comp>>>(sa);
       MCK(cudaMemcpyAsync(a->h_ctr_pinned, ctr, sizeof(Counters), cudaMemcpyDeviceToHost, a->s_comp));
       if ((rc = store_ctl_read(a, &ctl))) return g->fail(rc, a->err);
@@ -996,15 +1020,18 @@ static int merge_process(pa_merge* g) {
   StreamShare share(g);
   auto restore = [] {};
   // ---- rows of every shard -> global row ranges; registrations must be identical (ids are global)
-  struct Dims { uint64_t n, nf, store_entries, store_frames, n_stack_frames, stack_digest; uint32_t ncols, nlab, n_frames, n_cstr, n_labelsets, n_funcs, lz4, schema, group_stacks, n_stacks; };
+  // (group retire: n_stack_frames is the frames of the stacks not yet freed, since dead frames make arena lengths differ)
+  struct Dims { uint64_t n, nf, store_entries, store_frames, n_stack_frames, stack_digest, stages;
+                uint32_t ncols, nlab, n_frames, n_cstr, n_labelsets, n_funcs, lz4, schema, group_stacks, n_stacks, group_retire; };
   std::vector<const void*> src(L);
   std::vector<uint8_t> hb;
   rc = PA_OK;
   for (size_t i = 0; i < L && !rc; i++) {
     pa_agg* a = g->members[i];
     cudaSetDevice(a->device);
-    Dims d{a->N, a->NF, a->store_entries, a->store_frames, a->P.n_stack_frames, a->P.stack_digest, (uint32_t)a->cols.size(), a->n_label_cols, a->P.n_frames,
-           a->P.n_cstr, a->P.n_labelsets, a->P.n_funcs, g->lz4 ? 1u : 0u, (uint32_t)a->cfg.schema, a->group_stacks ? 1u : 0u, a->P.n_stacks};
+    Dims d{a->N, a->NF, a->store_entries, a->store_frames, a->group_retire ? a->P.stack_frames_live : a->P.n_stack_frames, a->P.stack_digest,
+           a->group_retire ? a->rs_stages : 0, (uint32_t)a->cols.size(), a->n_label_cols, a->P.n_frames, a->P.n_cstr, a->P.n_labelsets, a->P.n_funcs,
+           g->lz4 ? 1u : 0u, (uint32_t)a->cfg.schema, a->group_stacks ? 1u : 0u, a->P.n_stacks, a->group_retire ? 1u : 0u};
     if (g->mb[i].gather_scratch.ensure(std::max<size_t>((size_t)(W + 1) * sizeof(Dims), 256)) != cudaSuccess) { rc = g->fail(PA_ENOMEM, "device allocation failed"); break; }
     // staged through the tail of the gather scratch (the head receives the gathered block)
     uint8_t* mine = g->mb[i].gather_scratch.as<uint8_t>() + (size_t)W * sizeof(Dims);
@@ -1017,9 +1044,11 @@ static int merge_process(pa_merge* g) {
   for (uint32_t r = 0; r < W; r++) {  // one member per process: the group's modes are settled here, before any work
     if (dims[r].lz4 != dims[0].lz4) { restore(); return g->fail(PA_EINVAL, kLz4Mixed); }
     if (dims[r].schema != dims[0].schema) { restore(); return g->fail(PA_EINVAL, kSchemaMixed); }
+    const bool differ = dims[r].n_stacks != dims[0].n_stacks || dims[r].n_stack_frames != dims[0].n_stack_frames || dims[r].stack_digest != dims[0].stack_digest;
     const char* why = dims[r].group_stacks != dims[0].group_stacks ? kStacksMixed
-                    : dims[0].group_stacks && (dims[r].n_stacks != dims[0].n_stacks || dims[r].n_stack_frames != dims[0].n_stack_frames ||
-                                               dims[r].stack_digest != dims[0].stack_digest) ? kStacksMismatch : nullptr;
+                    : dims[r].group_retire != dims[0].group_retire ? kRetireMixed
+                    : dims[0].group_retire && (differ || dims[r].stages != dims[0].stages) ? kRetireMismatch
+                    : dims[0].group_stacks && differ ? kStacksMismatch : nullptr;
     if (why) {  // (also where the caller of each local member looks for it)
       restore();
       for (pa_agg* m : g->members) m->fail(PA_EINVAL, why);
@@ -1032,6 +1061,7 @@ static int merge_process(pa_merge* g) {
   }
   const bool v1 = dims[0].schema == PA_SCHEMA_V1;
   g->group_stacks = dims[0].group_stacks != 0;
+  g->group_retire = dims[0].group_retire != 0;
   g->n_rows.assign(W, 0); g->nf.assign(W, 0); g->row_base.assign(W + 1, 0);
   g->NT = 0; g->NFT = 0;
   for (uint32_t r = 0; r < W; r++) {
@@ -1044,7 +1074,8 @@ static int merge_process(pa_merge* g) {
   }
   g->row_base[W] = g->NT;
   // group stacks: the rings hold no frames; the merged location-index stream, and each shard's slice of it, is bounded by the
-  // (identical) registered arena, as one registered-stacks aggregator's is
+  // (identical) registered arena, as one registered-stacks aggregator's is; with group retire by the frames of the stacks not yet
+  // freed, which every stack a row may name belongs to
   if (g->group_stacks) g->NFT = dims[0].n_stack_frames;
   g->ncols = dims[0].ncols;
   if (g->NT > 0x7FFFFFFFull) { restore(); return g->fail(PA_ERANGE, "merged batch exceeds the int32 row limit of run ends / ListView offsets"); }
@@ -1664,6 +1695,12 @@ int pa_merge_create_local(pa_agg* const* members, uint32_t n, pa_merge** out) {
     return PA_EINVAL;
   }
   if (any_registered) return PA_EINVAL;
+  uint32_t n_retire = 0;
+  for (uint32_t i = 0; i < n; i++) n_retire += members[i]->group_retire;
+  if (n_retire && n_retire != n) {
+    for (uint32_t i = 0; i < n; i++) members[i]->fail(PA_EINVAL, kRetireMixed);
+    return PA_EINVAL;
+  }
   if (n_lz4 && n_lz4 != n) {  // the reason goes where the caller of a PA_IPC_LZ4_FRAME_GPU member looks for it
     for (uint32_t i = 0; i < n; i++) if (lz4_gpu_member(members[i])) members[i]->fail(PA_EINVAL, kLz4Mixed);
     return PA_EINVAL;
@@ -1808,6 +1845,76 @@ void pa_merge_destroy(pa_merge* g) {
 }
 const char* pa_merge_last_error(const pa_merge* g) { return g ? g->err.c_str() : "null handle"; }
 
+// PA_CFG_GROUP_RETIRE: pa_agg_retire_stacks for the whole group. The arguments and each member's state go round first, so that a
+// refusal is taken on every rank before any other collective. Then each slot's last_use becomes the group's maximum (inverted
+// around an all-reduce(min): a slot the emit marked 0xFFFFFFFF inverts to 0 and stays marked), and every member runs the single
+// aggregator's selection and bookkeeping on identical inputs, so every member retires the same slots.
+static const char kRetireRefused[] = "pa_merge_retire_stacks needs, on every rank, PA_CFG_GROUP_RETIRE members whose staged batch is collected, "
+                                     "idle_batches >= 1, and the same idle_batches, cap, stage count and uploaded slot count";
+static int merge_retire_stacks(pa_merge* g, uint32_t idle, uint64_t* handles, uint64_t cap, uint64_t* n_retired) {
+  const size_t L = g->members.size();
+  const uint32_t W = g->world;
+  if (n_retired) *n_retired = 0;
+  StreamShare share(g);
+  struct RetireDims { uint64_t cap, stages, slots; uint32_t idle, ok; };
+  std::vector<const void*> src(L);
+  for (size_t i = 0; i < L; i++) {
+    pa_agg* a = g->members[i];
+    MCK(cudaSetDevice(a->device));
+    const RetireDims d{cap, a->rs_stages, a->rs_dev_slots, idle, a->group_retire && a->staged < 0 && idle > 0 && (handles || !cap) ? 1u : 0u};
+    MCK(g->mb[i].gather_scratch.ensure(std::max<size_t>((size_t)(W + 1) * sizeof(RetireDims), 256)));
+    uint8_t* mine = g->mb[i].gather_scratch.as<uint8_t>() + (size_t)W * sizeof(RetireDims);  // (behind the gathered block, as in merge_process)
+    MCK(cudaMemcpyAsync(mine, &d, sizeof d, cudaMemcpyHostToDevice, a->s_comp));
+    MCK(cudaStreamSynchronize(a->s_comp));
+    src[i] = mine;
+  }
+  std::vector<uint8_t> hb;
+  int rc = t_allgather_host(g, src, sizeof(RetireDims), hb);
+  if (rc) return rc;
+  const RetireDims* d = (const RetireDims*)hb.data();
+  for (uint32_t r = 0; r < W; r++)
+    if (!d[r].ok || d[r].idle != d[0].idle || d[r].cap != d[0].cap || d[r].stages != d[0].stages || d[r].slots != d[0].slots) {
+      for (pa_agg* m : g->members) m->fail(PA_EINVAL, kRetireRefused);
+      return g->fail(PA_EINVAL, kRetireRefused);
+    }
+  const uint64_t ns = d[0].slots;
+  if (d[0].stages >= idle && ns && cap) {  // (otherwise retire_stacks selects nothing, on every rank alike)
+    std::vector<uint32_t*> last(L);
+    for (size_t i = 0; i < L; i++) {
+      pa_agg* a = g->members[i];
+      MCK(cudaSetDevice(a->device));
+      last[i] = a->d_rs_last.as<uint32_t>();
+      k_invert_u32<<<small_grid(a, ns), kThreads, 0, a->s_comp>>>(last[i], ns);
+    }
+    rc = t_allreduce_min(g, last, ns);
+    // inverted back on a failed reduction too: every word then holds a batch number this member or another one recorded, so no
+    // slot reads as idle longer than it is
+    for (size_t i = 0; i < L; i++) {
+      pa_agg* a = g->members[i];
+      MCK(cudaSetDevice(a->device));
+      k_invert_u32<<<small_grid(a, ns), kThreads, 0, a->s_comp>>>(last[i], ns);
+    }
+    if (rc) return rc;
+  }
+  std::vector<uint64_t> other(cap ? std::min<uint64_t>(cap, ns) : 0);
+  uint64_t n0 = 0;
+  for (size_t i = 0; i < L; i++) {
+    pa_agg* a = g->members[i];
+    uint64_t* h = i == 0 ? handles : other.data();
+    uint64_t n = 0;
+    if ((rc = retire_stacks(a, idle, h, cap, &n))) return g->fail(rc, a->err);
+    if (i == 0) n0 = n;
+    else if (n != n0 || !std::equal(h, h + n, handles)) return g->fail(PA_EIO, "the members of a PA_CFG_GROUP_RETIRE group selected different stacks to retire");
+    std::lock_guard<std::mutex> lk(a->reg_mu);  // every retirement is digested too (idle_batches, then the handles), apart from registrations
+    std::vector<uint64_t> wide(1 + n);
+    wide[0] = idle;
+    std::copy(h, h + n, wide.begin() + 1);
+    a->retire_digest = pa_xxh64(wide.data(), wide.size() * 8, a->retire_digest);
+  }
+  if (n_retired) *n_retired = n0;
+  return PA_OK;
+}
+
 namespace {
 struct MergeLocks {  // the members' flush locks, taken in member order
   std::vector<std::unique_lock<std::mutex>> l;
@@ -1843,6 +1950,11 @@ int pa_merge_flush(pa_merge* g, pa_agg_result* out) {
   if ((rc = merge_plan(g, &len))) { drop(); return rc; }
   if ((rc = merge_collect(g, nullptr, 0, out))) drop();
   return rc;
+}
+int pa_merge_retire_stacks(pa_merge* g, uint32_t idle_batches, uint64_t* handles, uint64_t cap, uint64_t* n_retired) {
+  if (!g) return PA_EINVAL;
+  MergeLocks lk(g);
+  return merge_retire_stacks(g, idle_batches, handles, cap, n_retired);
 }
 int pa_merge_stacktraces(pa_merge* g, const uint8_t* ids, uint64_t n_ids, pa_agg_result* out) {
   if (!g || !out) return PA_EINVAL;

@@ -21,7 +21,7 @@ EXPORTS = [
     "pa_agg_debug_stack_ids", "pa_agg_debug_stack_counts", "pa_agg_debug_pair_counts", "pa_agg_stacktraces", "pa_agg_last_stack_ids", "pa_agg_shard_sizes", "pa_agg_shard_export", "pa_agg_stage_device", "pa_agg_stage_device_parts", "pa_agg_discard", "pa_ipc_compress_lz4", "pa_ipc_free", "pa_fix_truncation", "pa_xxh64",
     "pa_merge_create_local", "pa_merge_nccl_unique_id", "pa_merge_create_nccl", "pa_merge_destroy", "pa_merge_last_error", "pa_merge_process",
     "pa_merge_plan", "pa_merge_collect", "pa_merge_flush", "pa_merge_last_stats", "pa_merge_create_host", "pa_merge_create_shm",
-    "pa_merge_stacktraces", "pa_agg_register_stack_handles", "pa_agg_retire_stacks",
+    "pa_merge_stacktraces", "pa_agg_register_stack_handles", "pa_agg_retire_stacks", "pa_merge_retire_stacks",
 ]
 
 
@@ -51,6 +51,7 @@ def lib():
         L.pa_agg_register_stacks.argtypes = [vp, vp, vp, vp, C.c_uint32, u64p]
         L.pa_agg_register_stack_handles.argtypes = [vp, vp, vp, vp, C.c_uint32, vp]
         L.pa_agg_retire_stacks.argtypes = [vp, C.c_uint32, vp, C.c_uint64, u64p]
+        L.pa_merge_retire_stacks.argtypes = [vp, C.c_uint32, vp, C.c_uint64, u64p]
         L.pa_agg_acquire.argtypes = [vp, C.c_uint64, C.c_uint64, C.POINTER(vp), C.POINTER(vp), u64p]
         L.pa_agg_commit.argtypes = [vp, C.c_uint64]
         L.pa_agg_submit.argtypes = [vp, vp, vp, C.c_uint64]
@@ -398,6 +399,21 @@ class MergeGroup:
         self._ck(lib().pa_merge_stacktraces(self.h, ids or None, len(ids) // 16, C.byref(raw)))
         return Result(raw)
 
+    def retire_stacks(self, idle_batches, cap=None):
+        """PA_CFG_GROUP_RETIRE groups (collective, after collect): retire the stacks no member named for `idle_batches` batches
+        (at most `cap`, default all); returns their handles in slot order, the same on every rank. Drop them from the lookup
+        before the next interval. The default cap is the same on every rank (ranks must agree on it); the handle buffer is
+        sized by this member's slots, never fewer than the uploaded slots the call selects from."""
+        if cap is None:
+            c = self.members[0].stack_counters()
+            cap, room = 2**64 - 1, c["stacks_live"] + c["stacks_free"]
+        else:
+            room = cap
+        out = np.zeros(max(room, 1), dtype=np.uint64)
+        n = C.c_uint64()
+        self._ck(lib().pa_merge_retire_stacks(self.h, idle_batches, out.ctypes.data, cap, C.byref(n)))
+        return out[:n.value]
+
     def stats(self):
         wall, wait, nb, nr = C.c_double(), C.c_double(), C.c_uint64(), C.c_uint64()
         self._ck(lib().pa_merge_last_stats(self.h, C.byref(wall), C.byref(wait), C.byref(nb), C.byref(nr)))
@@ -517,14 +533,16 @@ def expand_stack_form(hdrs, sf):
     return hd, np.asarray(sf.frames, dtype=np.uint64)[idx]
 
 
-def from_workload(w, device=0, max_samples=None, max_frames=None, chunk_samples=0, registered_stacks=False, group_form=None, flags=0, **kw):
+def from_workload(w, device=0, max_samples=None, max_frames=None, chunk_samples=0, registered_stacks=False, group_form=None, group_retire=False,
+                  flags=0, **kw):
     """Aggregator with the workload's dictionaries registered (string id 0 == "" is implicit). registered_stacks: a
     PA_CFG_REGISTERED_STACKS aggregator with the workload's stacks registered too (stack_form); max_frames then defaults to
     the registered frames. group_form: a PA_CFG_REGISTERED_STACKS | PA_CFG_GROUP_STACKS aggregator that registers this
-    StackForm (group_stack_form) instead, as every member of its merge group does."""
+    StackForm (group_stack_form) instead, as every member of its merge group does; with group_retire, PA_CFG_GROUP_RETIRE too
+    (a fresh registry hands out handles equal to the form's stack numbers)."""
     sf = group_form if group_form is not None else stack_form(w) if registered_stacks else None
     if group_form is not None:
-        flags |= abi.PA_CFG_REGISTERED_STACKS | abi.PA_CFG_GROUP_STACKS
+        flags |= abi.PA_CFG_REGISTERED_STACKS | abi.PA_CFG_GROUP_STACKS | (abi.PA_CFG_GROUP_RETIRE if group_retire else 0)
     n = max(1, w.n if max_samples is None else max_samples)
     nf = max(1, (len(sf.frames) if sf else w.n_frame_ids) if max_frames is None else max_frames)
     a = Aggregator(device=device, hash_mode=w.hash_mode, label_flags=w.label_flags, samples_per_second=w.samples_per_second,

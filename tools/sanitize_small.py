@@ -2,7 +2,7 @@
 added in round 2 — early copy-out during a multi-chunk flush, the v1 LRU store (evictions, revivals, compaction, over-full batch),
 the pipelined / bulk-copy-staged hash variants, the narrow ring, a 3-shard merged record.
 
-usage: PA_EARLY_D2H_ALWAYS=1 compute-sanitizer --tool memcheck python tools/sanitize_small.py [plain|lz4_gpu|merge_lz4_gpu|merge_v1|registered|merge_group_stacks]
+usage: PA_EARLY_D2H_ALWAYS=1 compute-sanitizer --tool memcheck python tools/sanitize_small.py [plain|lz4_gpu|merge_lz4_gpu|merge_v1|registered|merge_group_stacks|merge_group_retire]
 lz4_gpu: small flushes with the bodies compressed on the device (PA_IPC_LZ4_FRAME_GPU) instead: a multi-chunk v2 batch, the
 narrow ring, and a v1 batch with its stacktrace record, each checked against the oracle's plain stream.
 merge_lz4_gpu: a small in-process merge group of PA_IPC_LZ4_FRAME_GPU members whose shard cuts put blocks across part borders
@@ -13,7 +13,10 @@ registered: PA_CFG_REGISTERED_STACKS aggregators (both hash modes, the narrow ri
 row naming an unregistered stack id followed by a clean flush.
 merge_group_stacks: in-process groups of PA_CFG_GROUP_STACKS members — a v2 interval over three shards with an empty one, and
 v1 intervals against a small store (stack references instead of frames), checked against one group-stacks aggregator, a ring
-group and the oracle."""
+group and the oracle.
+merge_group_retire: in-process groups of PA_CFG_GROUP_RETIRE members through a small churn (v2 over three shards, v1 over two):
+retirement with the group-wide last_use, re-registration into freed slots, compaction, and v1 store references as handles,
+checked against one PA_CFG_RETIRE_STACKS aggregator."""
 import os
 import sys
 
@@ -115,8 +118,31 @@ def merge_group_stacks():
     print("sanitize_small merge_group_stacks ok")
 
 
+def merge_group_retire():
+    from test_merge_group_retire import GroupChurn
+    from test_stack_retirement import windows
+    for world, schema in ((3, abi.PA_SCHEMA_V2), (2, abi.PA_SCHEMA_V1)):
+        w = synth.ragged(n=3000, u=600, p=1024, max_depth=40, hash_mode=abi.PA_HASH_XXH64X2)
+        w.schema = schema
+        c = GroupChurn(w, world, max_frames=200_000, max_samples=600, stack_cache_entries=150 if schema == abi.PA_SCHEMA_V1 else 0)
+        ws = windows(len(c.sf.hashes), 200, 60, 7)
+        for k in range(6):
+            hdrs, stacks = c.rows(ws[k], 500)
+            r, r1 = c.flush(hdrs, stacks, k)
+            assert r.ipc_bytes() == r1.ipc_bytes()
+            if schema == abi.PA_SCHEMA_V1:
+                ids = c.single.last_stack_ids(r1.n_unique_stacks).tobytes()
+                assert c.g.stacktraces(ids).ipc_bytes() == c.single.stacktraces(ids).ipc_bytes()
+            c.retire(1)
+            c.check_counters()
+        c.close()
+    print("sanitize_small merge_group_retire ok")
+
+
 def main():
     oracle_py.build()
+    if sys.argv[1:] == ["merge_group_retire"]:
+        return merge_group_retire()
     if sys.argv[1:] == ["merge_group_stacks"]:
         return merge_group_stacks()
     if sys.argv[1:] == ["registered"]:
