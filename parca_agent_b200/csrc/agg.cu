@@ -106,10 +106,10 @@ struct MergeDims { uint32_t world = 1, rank = 0; uint64_t row_base = 0, n_total 
 struct Pass {
   // registration state as mirrored to the device for this batch (snapshot taken under reg_mu in upload_tables)
   uint32_t n_cstr = 0, n_frames = 0, n_funcs = 0, n_sids = 0, n_labelsets = 0;
-  uint32_t n_stacks = 0;          // registered stacks (PA_CFG_REGISTERED_STACKS)
-  uint64_t n_stack_frames = 0;    // and the frame ids of their arena
+  uint32_t n_stacks = 0;          // stack slots on the device (PA_CFG_REGISTERED_STACKS)
+  uint64_t n_stack_frames = 0;    // and the frame ids of their arena (freed stacks' included until a compaction)
   uint64_t stack_digest = 0;      // PA_CFG_GROUP_STACKS: digest of those stacks (merge groups check it is the same on every member)
-  uint64_t stack_frames_live = 0; // PA_CFG_GROUP_RETIRE: frames of the uploaded stacks not yet freed (the same on every member)
+  uint64_t stack_frames_live = 0; // frames of the uploaded stacks not yet freed (in a merge group, the same on every member)
   uint64_t N = 0, NT = 0, row_base = 0;
   uint32_t world = 1, rank = 0, ncols = 0, nlab = 0;
   bool v1 = false, provided = false, merged = false;  // provided: the stack ids arrive with the rows (or their registered stacks)
@@ -185,23 +185,19 @@ struct pa_agg {
   Mirror<uint64_t> m_addr, m_line;
   Mirror<uint32_t> m_type, m_map, m_bid, m_func, m_fnfile, m_sid2cid;
   DBuf d_lsmat, d_kindtab, d_cols, d_jobs;
-  // PA_CFG_REGISTERED_STACKS: the registered stacks and their frame arena (ids at the ring's width, idb / 4 words each)
+  // PA_CFG_REGISTERED_STACKS: the stack registry. The device holds it (records, last_use, the frame arena with ids at the ring's
+  // width, idb / 4 words each). The host keeps per-slot metadata, the free slots (a min-heap), the retired stacks waiting for
+  // their grace batch, and the registrations not yet uploaded. Without PA_CFG_RETIRE_STACKS no slot is ever freed, so every
+  // stack takes the next slot with generation 0 and its handle is its consecutive id.
   bool registered = false;
   bool group_stacks = false;  // PA_CFG_GROUP_STACKS: the stack ids are group-wide (merge groups)
-  uint64_t reg_digest = 0;    // PA_CFG_GROUP_STACKS: running digest of every registered stack's (id, depth, frame ids); with
-                              // PA_CFG_GROUP_RETIRE of (handle, id, depth, frame ids)
+  uint64_t reg_digest = 0;    // PA_CFG_GROUP_STACKS: running digest of every registered stack's (handle, id, depth, frame ids)
   // PA_CFG_GROUP_RETIRE: running digest of every group retirement's (idle_batches, handles), kept apart from reg_digest so that a
   // registration running concurrently with pa_merge_retire_stacks may land before or after it on each member; rs_upload combines
   // the two
   uint64_t retire_digest = 0;
-  std::vector<RegStack> reg_stacks;
-  std::vector<uint32_t> reg_arena;
-  Mirror<RegStack> m_stacks;
-  Mirror<uint32_t> m_arena;
-  // PA_CFG_RETIRE_STACKS: the device holds the registry (records, last_use, the frame arena). The host keeps per-slot metadata,
-  // the free slots (a min-heap), the retired stacks waiting for their grace batch, and the registrations not yet uploaded.
   enum : uint8_t { RS_LIVE, RS_RETIRING, RS_FREE };
-  bool retire = false;
+  bool retire = false;  // PA_CFG_RETIRE_STACKS: stacks can be retired and their slots reused
   bool group_retire = false;  // PA_CFG_GROUP_RETIRE (retire is set too): the merge group retires, through pa_merge_retire_stacks
   std::vector<uint32_t> rs_depth, rs_gen;  // rs_gen: the generation of the slot's current (or next) stack
   std::vector<uint8_t> rs_state;
@@ -226,7 +222,7 @@ struct pa_agg {
   uint32_t* h_select = nullptr;              // pinned: 256-bin histogram of a select pass, then a StoreCtl read-back
   uint64_t store_compactions = 0, store_evictions = 0;
   uint64_t store_frames_sent = 0;            // v1 merge groups: frame ids this member sent in the last store exchange
-  uint64_t store_refs_sent = 0;              // v1 PA_CFG_GROUP_STACKS merge groups: the arena offsets it sent instead
+  uint64_t store_refs_sent = 0;              // v1 PA_CFG_GROUP_STACKS merge groups: the stack handles it sent instead
   uint32_t cid_unknown = 0, cid_missing = 0;  // "unknown" (libpf.UnknownFrame.String()) and "missing stacktrace" (:1561, :1568)
 
   // ---- ring (pinned host), double buffered
@@ -492,7 +488,7 @@ int pa_agg_create(const pa_agg_config* cfg, pa_agg** out) {
   cudaEventCreate(&a->ev_d2h0);
   cudaEventCreate(&a->ev_d2h1);
   for (int t = 0; t < T_COUNT; t++) { cudaEventCreate(&a->tm[t].a); cudaEventCreate(&a->tm[t].b); }
-  if (a->retire) { cudaEventCreate(&a->rs_tm.a); cudaEventCreate(&a->rs_tm.b); }
+  if (a->registered) { cudaEventCreate(&a->rs_tm.a); cudaEventCreate(&a->rs_tm.b); }
   if (a->cfg.ipc_compression == PA_IPC_LZ4_FRAME_GPU) { cudaEventCreate(&a->ev_lz4p0); cudaEventCreate(&a->ev_lz4p1); }
   const uint64_t N = a->cfg.max_samples, NF = a->cfg.max_frames;
   if (a->idb == 4 && a->hash_variant != 5) a->hash_variant = 2;  // (the tma variants fall through to wide32 in launch_hash)  // the narrow ring is read by the `wide` kernel (widening loads); the other variants take uint64 ids
@@ -561,7 +557,7 @@ void pa_agg_destroy(pa_agg* a) {
   DBuf* all[] = {&a->d_hdr, &a->d_frames, &a->d_ts, &a->d_value, &a->d_uuid, &a->d_stoff, &a->d_stsize, &a->d_slot, &a->d_kind, &a->d_nfr,
                  &a->d_foff, &a->d_ls, &a->d_cpu, &a->d_tid, &a->d_comm, &a->d_ustream, &a->d_uniq_row, &a->d_uniq_count, &a->d_table, &a->d_ctr,
                  &a->d_arena, &a->d_partial, &a->d_partial2, &a->d_ree_partial, &a->d_lsmat, &a->d_kindtab, &a->d_cols, &a->d_jobs,
-                 &a->m_stacks.buf, &a->m_arena.buf, &a->m_addr.buf, &a->m_line.buf, &a->m_type.buf, &a->m_map.buf, &a->m_bid.buf, &a->m_func.buf, &a->m_fnfile.buf, &a->m_sid2cid.buf,
+                 &a->m_addr.buf, &a->m_line.buf, &a->m_type.buf, &a->m_map.buf, &a->m_bid.buf, &a->m_func.buf, &a->m_fnfile.buf, &a->m_sid2cid.buf,
                  &a->m1_map.buf, &a->m1_bid.buf, &a->m1_fn.buf, &a->m1_file.buf, &a->m1_line.buf, &a->m1_col.buf, &a->m1_complete.buf,
                  &a->d_store, &a->d_store_arena, &a->d_store_ctl, &a->d_v1_ids, &a->d_st1, &a->d_store_stamp, &a->d_v1_last, &a->d_select, &a->d_lz4, &a->d_lz4_body,
                  &a->d_rs_recs, &a->d_rs_last, &a->d_rs_arena[0], &a->d_rs_arena[1], &a->d_rs_tmp, &a->d_rs_upd};
@@ -623,7 +619,7 @@ int pa_agg_register_labelsets(pa_agg* a, const pa_label_pair* pairs, const uint3
   return PA_OK;
 }
 // Validation shared by both registration calls (a refused call registers nothing). check_stack_args runs before reg_mu is
-// taken, check_stack_shape and check_stack_frames under it, with the mode's space check in between.
+// taken, check_stack_shape and check_stack_frames under it, with the space checks in between.
 static int check_stack_args(pa_agg* a, const uint64_t* hashes, const uint64_t* offsets, uint32_t n, const char* fn) {
   if (!a->registered) return a->fail(PA_EINVAL, (std::string(fn) + " needs an aggregator created with PA_CFG_REGISTERED_STACKS").c_str());
   if (n && !offsets) return PA_EINVAL;
@@ -668,57 +664,17 @@ static void stack_key(const pa_agg* a, const uint64_t* hashes, const uint64_t* f
   s->hash_lo = pa_xxh64(wide.data(), d * 8, PA_XXH_SEED_LO);
 }
 
-int pa_agg_register_stacks(pa_agg* a, const uint64_t* hashes, const uint64_t* frames, const uint64_t* offsets, uint32_t n, uint64_t* first_stack_id) {
-  if (!a) return PA_EINVAL;
-  int rc = check_stack_args(a, hashes, offsets, n, "pa_agg_register_stacks");
-  if (rc) return rc;
-  if (a->retire) return a->fail(PA_EINVAL, "PA_CFG_RETIRE_STACKS: register through pa_agg_register_stack_handles");
-  std::lock_guard<std::mutex> g(a->reg_mu);
-  const uint64_t words = a->idb / 4;
-  const uint64_t have = a->reg_arena.size() / words;
-  uint64_t total = 0;
-  if ((rc = check_stack_shape(a, frames, offsets, n, &total))) return rc;
-  if (have + total > a->cfg.max_frames) return a->fail(PA_ENOSPC, "registered frames would exceed max_frames");
-  if (a->reg_stacks.size() + n > 0xFFFFFFFFull) return a->fail(PA_ENOSPC, "more than 2^32 - 1 registered stacks");  // (ids are checked as uint32 on the device)
-  const uint32_t* f32 = (const uint32_t*)frames;
-  if ((rc = check_stack_frames(a, frames, offsets, n))) return rc;
-  if (first_stack_id) *first_stack_id = a->reg_stacks.size();
-  std::vector<uint64_t> wide;
-  for (uint32_t i = 0; i < n; i++) {
-    const uint64_t d = offsets[i + 1] - offsets[i];
-    RegStack s{};
-    s.off = a->reg_arena.size() / words;
-    s.depth = (uint32_t)d;
-    const uint8_t* src = (const uint8_t*)frames + offsets[i] * a->idb;
-    a->reg_arena.resize(a->reg_arena.size() + d * words);
-    if (d) memcpy(a->reg_arena.data() + s.off * words, src, d * a->idb);
-    stack_key(a, hashes, frames, offsets, i, &s, wide);
-    if (a->group_stacks) {  // the registry's digest: XXH64 of (hash_hi, hash_lo, depth, frame ids as uint64), seeded with the digest so far
-      wide.resize(d + 3);
-      wide[0] = s.hash_hi; wide[1] = s.hash_lo; wide[2] = d;
-      for (uint64_t j = 0; j < d; j++) wide[3 + j] = a->idb == 4 ? (uint64_t)f32[offsets[i] + j] : frames[offsets[i] + j];
-      a->reg_digest = pa_xxh64(wide.data(), (d + 3) * 8, a->reg_digest);
-    }
-    a->reg_stacks.push_back(s);
-  }
-  return PA_OK;
-}
-int pa_agg_register_stack_handles(pa_agg* a, const uint64_t* hashes, const uint64_t* frames, const uint64_t* offsets, uint32_t n, uint64_t* handles) {
-  if (!a || (n && !handles)) return PA_EINVAL;
-  if (!a->retire) {
-    uint64_t first = 0;
-    int rc = pa_agg_register_stacks(a, hashes, frames, offsets, n, &first);
-    for (uint32_t i = 0; i < n && !rc; i++) handles[i] = first + i;
-    return rc;
-  }
-  int rc = check_stack_args(a, hashes, offsets, n, "pa_agg_register_stack_handles");
-  if (rc) return rc;
+// Both registration calls, after check_stack_args: each stack takes the lowest free slot, or a new one. `handles` (if not null)
+// receives generation << 32 | slot for each stack, `first_slot` (if not null) the slot count before the call.
+static int register_stacks(pa_agg* a, const uint64_t* hashes, const uint64_t* frames, const uint64_t* offsets, uint32_t n, uint64_t* handles, uint64_t* first_slot) {
   std::lock_guard<std::mutex> g(a->reg_mu);
   uint64_t total = 0;
+  int rc;
   if ((rc = check_stack_shape(a, frames, offsets, n, &total))) return rc;
   if (a->rs_frames_live + total > a->cfg.max_frames) return a->fail(PA_ENOSPC, "live registered frames would exceed max_frames");
   if (n > a->rs_free.size() && a->rs_state.size() + (n - a->rs_free.size()) > 0xFFFFFFFFull) return a->fail(PA_ENOSPC, "more than 2^32 - 1 stack slots");
   if ((rc = check_stack_frames(a, frames, offsets, n))) return rc;
+  if (first_slot) *first_slot = a->rs_state.size();
   const uint64_t words = a->idb / 4;
   std::vector<uint64_t> wide;
   for (uint32_t i = 0; i < n; i++) {
@@ -742,15 +698,30 @@ int pa_agg_register_stack_handles(pa_agg* a, const uint64_t* hashes, const uint6
     a->rs_pend.push_back(s); a->rs_pend_slot.push_back(slot); a->rs_pend_seq.push_back((uint32_t)a->rs_stages);
     a->rs_state[slot] = pa_agg::RS_LIVE; a->rs_depth[slot] = (uint32_t)d;
     a->rs_live++; a->rs_frames_live += d;
-    handles[i] = ((uint64_t)a->rs_gen[slot] << 32) | slot;
-    if (a->group_retire) {  // the registry's digest, as for PA_CFG_GROUP_STACKS with the handle in front
+    const uint64_t handle = ((uint64_t)a->rs_gen[slot] << 32) | slot;
+    if (handles) handles[i] = handle;
+    if (a->group_stacks) {  // the registry's digest: XXH64 of (handle, hash_hi, hash_lo, depth, frame ids as uint64), seeded with the digest so far
       wide.resize(d + 4);
-      wide[0] = handles[i]; wide[1] = s.hash_hi; wide[2] = s.hash_lo; wide[3] = d;
+      wide[0] = handle; wide[1] = s.hash_hi; wide[2] = s.hash_lo; wide[3] = d;
       for (uint64_t j = 0; j < d; j++) wide[4 + j] = a->idb == 4 ? (uint64_t)((const uint32_t*)frames)[offsets[i] + j] : frames[offsets[i] + j];
       a->reg_digest = pa_xxh64(wide.data(), (d + 4) * 8, a->reg_digest);
     }
   }
   return PA_OK;
+}
+
+int pa_agg_register_stacks(pa_agg* a, const uint64_t* hashes, const uint64_t* frames, const uint64_t* offsets, uint32_t n, uint64_t* first_stack_id) {
+  if (!a) return PA_EINVAL;
+  int rc = check_stack_args(a, hashes, offsets, n, "pa_agg_register_stacks");
+  if (rc) return rc;
+  if (a->retire) return a->fail(PA_EINVAL, "PA_CFG_RETIRE_STACKS: register through pa_agg_register_stack_handles");
+  return register_stacks(a, hashes, frames, offsets, n, nullptr, first_stack_id);  // (no slot is ever freed: the ids are consecutive)
+}
+int pa_agg_register_stack_handles(pa_agg* a, const uint64_t* hashes, const uint64_t* frames, const uint64_t* offsets, uint32_t n, uint64_t* handles) {
+  if (!a || (n && !handles)) return PA_EINVAL;
+  int rc = check_stack_args(a, hashes, offsets, n, "pa_agg_register_stack_handles");
+  if (rc) return rc;
+  return register_stacks(a, hashes, frames, offsets, n, handles, nullptr);
 }
 
 // ---- ingest ----------------------------------------------------------------------------------
@@ -825,7 +796,7 @@ static int stage_async(pa_agg* a) {
       a->ring[a->active].nfr = 0;
     }
   }
-  if (a->retire) {
+  if (a->registered) {
     int rc = rs_stage(a);
     if (rc) { release_staged(a); return rc; }  // (a CUDA failure: the detached batch is dropped)
   }
@@ -913,9 +884,9 @@ static void launch_scan(pa_agg* a, F f, int njobs, Timer& t, int gx, cudaStream_
 // grid for a pass over at most `bound` elements: >= 2048 elements per CTA, never more than the full grid
 static int small_grid(const pa_agg* a, uint64_t bound) { return (int)std::max<uint64_t>(1, std::min<uint64_t>((uint64_t)a->G, (bound + 2047) / 2048)); }
 
-// PA_CFG_RETIRE_STACKS, under reg_mu, on the compute stream: applies `frees` (records with kStackFree, for free_slots), compacts
-// the arena when the dead frames outweigh the live ones (at a stage only: no batch is resident then) or when the pending frames
-// would not fit (a regrow, before the pass that reads the records), then uploads the pending registrations.
+// PA_CFG_REGISTERED_STACKS, under reg_mu, on the compute stream: applies `frees` (records with kStackFree, for free_slots),
+// compacts the arena when the dead frames outweigh the live ones (at a stage only: no batch is resident then) or when the
+// pending frames would not fit (a regrow, before the pass that reads the records), then uploads the pending registrations.
 static int rs_upload(pa_agg* a, const std::vector<RegStack>& frees, const std::vector<uint32_t>& free_slots, bool at_stage) {
   cudaStream_t s = a->s_comp;
   const uint64_t words = a->idb / 4, n_slots = a->rs_state.size();
@@ -988,6 +959,12 @@ static int rs_upload(pa_agg* a, const std::vector<RegStack>& frees, const std::v
     a->rs_pend.clear(); a->rs_pend_slot.clear(); a->rs_pend_seq.clear(); a->rs_pend_frames.clear();
   }
   CK(cudaGetLastError());
+  // A grow leaves the old arena allocated as the next compaction's target. A registry that never frees a slot never compacts,
+  // so it releases that arena after a grow, and the upload and compaction scratch the grown burst sized.
+  if (grow && !a->retire) {
+    CK(cudaStreamSynchronize(s));
+    a->d_rs_arena[a->rs_cur ^ 1].release(); a->d_rs_tmp.release(); a->d_rs_upd.release();
+  }
   a->rs_dev_slots = n_slots;
   a->src_frames = (const unsigned long long*)a->d_rs_arena[a->rs_cur].p;
   a->P.n_stacks = (uint32_t)n_slots;
@@ -1033,14 +1010,9 @@ static int upload_tables(pa_agg* a) {
     CK(a->m1_file.sync(a->ft.v1_file_cid, s)); CK(a->m1_line.sync(a->ft.v1_line, s)); CK(a->m1_col.sync(a->ft.v1_col, s));
     CK(a->m1_complete.sync(a->ft.v1_complete, s));
   }
-  if (a->retire) {
+  if (a->registered) {
     int rc = rs_upload(a, {}, {}, false);
     if (rc) return rc;
-  } else if (a->registered) {
-    CK(a->m_stacks.sync(a->reg_stacks, s)); CK(a->m_arena.sync(a->reg_arena, s));
-    a->src_frames = (const unsigned long long*)a->m_arena.ptr();  // (a regrown mirror moves: set on every upload)
-    a->P.n_stacks = (uint32_t)a->reg_stacks.size(); a->P.n_stack_frames = a->reg_arena.size() / (a->idb / 4);
-    a->P.stack_digest = a->reg_digest;
   }
   // what the device mirrors now hold: the pass uses these counts only (registration may continue concurrently)
   a->P.n_cstr = a->sp.count(); a->P.n_frames = a->ft.count(); a->P.n_funcs = a->ft.n_funcs();
@@ -1457,7 +1429,7 @@ static int pass_front(pa_agg* a) {
       if (a->cols[c].type == COL_COMM) h.first_comm = P.col_first[c];
     }
     h.first_kind = P.v1 ? a->v1_first_kind : nullptr;
-    h.stacks = (const uint4*)(a->retire ? a->d_rs_recs.p : a->m_stacks.ptr()); h.n_stacks = P.n_stacks;
+    h.stacks = (const uint4*)a->d_rs_recs.p; h.n_stacks = P.n_stacks;
     h.last_use = a->d_rs_last.as<uint32_t>(); h.seq = (uint32_t)a->rs_stages;
     uint64_t rows = r1 - r0;
     int hb = (int)std::min<uint64_t>((rows + kThreads - 1) / kThreads, (uint64_t)a->sms * kHdrBlocksPerSm);
@@ -3030,7 +3002,7 @@ int pa_agg_last_kernel_ms(const pa_agg* a, const char* name, double* ms, uint32_
     if (launches) *launches = a->rs_tm.launches;
     return PA_OK;
   }
-  // PA_SCHEMA_V1 merge groups of PA_CFG_GROUP_STACKS members (ms is 0): stack references (8-byte arena offsets) this member sent
+  // PA_SCHEMA_V1 merge groups of PA_CFG_GROUP_STACKS members (ms is 0): stack references (8-byte handles) this member sent
   // instead of frame ids in the last store exchange
   if (!strcmp(name, "store_refs")) {
     if (ms) *ms = 0;

@@ -272,8 +272,8 @@ struct HeaderArgs {
   uint32_t tid_mask;
   uint32_t* first_comm;
   uint32_t* first_kind;          // [8] first row of each sample kind (v1: the kind-derived columns are dictionary encoded)
-  const uint4* stacks;           // k_header<true>: the registered stack records (RegStack, two uint4 each)
-  uint32_t n_stacks;             // records mirrored for this batch
+  const uint4* stacks;           // k_header<true>: the registered stack records (RegStack, two uint4 each), one per slot
+  uint32_t n_stacks;             // records uploaded for this batch
   uint32_t* last_use;            // k_header<true, true>: per slot, the sequence number of the last batch that named it
   uint32_t seq;                  // this batch's sequence number (batches staged so far, this one included)
 };
@@ -285,13 +285,13 @@ struct HeaderArgs {
 // 2 KB of shared memory and at most 32 registers per thread keep all 64 warps of an SM resident, as many as these
 // latency-bound lookups want. The shared-memory carveout is left to the driver: the rest of L1 caches the small lookup
 // tables, and forcing the largest carveout made the pass about 30 % slower in provided-hash mode on an H100.
-// kRegistered (PA_CFG_REGISTERED_STACKS): frame_off names a registered stack; its 32-byte record supplies the stack id, the
-// depth and the arena offset, and hash_hi / hash_lo / nframes of the row are ignored. Launched with provided = 1.
-// kRetire (PA_CFG_RETIRE_STACKS): frame_off is a handle, generation << 32 | slot. The record must carry that generation and
-// not be free; the row's batch sequence number is then stored into the slot's last_use word, only when it differs: every row of
-// a batch would write the same value, and with Zipf-distributed stacks the stores to hot slots serialise in L2 (on an H100, each
-// step a new batch of 4M config-3 rows: +0.026 ms of header time over plain registered stacks, +0.235 ms with an unconditional
-// store; DESIGN section 7).
+// kRegistered (PA_CFG_REGISTERED_STACKS): frame_off is a stack handle, generation << 32 | slot. The slot's 32-byte record must
+// carry that generation and not be free; it supplies the stack id, the depth and the arena offset, and hash_hi / hash_lo /
+// nframes of the row are ignored. Launched with provided = 1.
+// kRetire (PA_CFG_RETIRE_STACKS): the row's batch sequence number is also stored into the slot's last_use word, only when it
+// differs: every row of a batch would write the same value, and with Zipf-distributed stacks the stores to hot slots serialise
+// in L2 (on an H100, each step a new batch of 4M config-3 rows: +0.026 ms of header time over plain registered stacks, +0.235 ms
+// with an unconditional store; DESIGN section 7).
 constexpr int kHdrBlocksPerSm = 8;
 
 template <bool kRegistered, bool kRetire = false>
@@ -362,6 +362,9 @@ __global__ void __launch_bounds__(kThreads, kHdrBlocksPerSm) k_header(HeaderArgs
           err |= ERR_BAD_STACK_ID; k = Key128{0ull, 0ull}; nfr = 0; foff = 0;
         }
       } else if (kRegistered) {
+        // Without retirement every record has generation 0 and no slot is free, so the handles the check above accepts are
+        // exactly those below the record count. Deciding that before the loads, not on the loaded generation, lets the
+        // record's L2 latency overlap the lookups that follow (branching on it cost 0.05-0.11 ms of header time on config 3).
         if (foff < a.n_stacks) {
           const uint4 s0 = __ldg(a.stacks + 2 * foff), s1 = __ldg(a.stacks + 2 * foff + 1);
           k.hi = ((unsigned long long)s0.y << 32) | s0.x;
@@ -2372,11 +2375,10 @@ struct StoreInsertArgs {
   const uint32_t* g_last_inv;        // [U] 0xFFFFFFFF - global last row
   const uint32_t* g_frames;          // frames of the stacks the store lacks, gathered from the shards that hold their first occurrence
   const unsigned long long* g_foff;  // [U + 1] where each ordinal's frames start in g_frames (an ordinal without frames there: equal neighbours)
-  // k_store_insert<true, true> (PA_CFG_GROUP_STACKS): g_foff indexes g_refs instead, one entry per stack; the frames are read from
-  // this member's own registered arena (`frames`), which is the same on every member
-  const unsigned long long* g_refs;  // arena offset of each needed stack's frames, from its global first occurrence
-  // k_store_insert<true, true, true> (PA_CFG_GROUP_RETIRE): g_refs holds handles, resolved through this member's own records, since
-  // the members' arenas may be laid out differently (compactions at different points of the registrations)
+  // k_store_insert<true, true> (PA_CFG_GROUP_STACKS): g_foff indexes g_refs instead, one entry per stack. Each is a handle, resolved
+  // through this member's own records (g_recs) into its own registered arena (`frames`): the handles are the same on every member,
+  // but the arenas may be laid out differently (PA_CFG_GROUP_RETIRE: compactions at different points of the registrations)
+  const unsigned long long* g_refs;  // handle of each needed stack, from its global first occurrence
   const uint4* g_recs;               // RegStack records, two uint4 each
   uint32_t n_recs;
 };
@@ -2421,9 +2423,9 @@ __global__ void __launch_bounds__(kThreads) k_store_kill(unsigned long long* sta
 }
 // one warp per unique stack of the batch (unique within the launch, so a key is claimed by at most one warp).
 // MERGED: one replica of a merge group's store; u is the merged ordinal, frames come from the gathered buffer.
-// REFS (with MERGED): frames come from the member's registered arena, at the gathered offset (g_refs).
-// HANDLES (with REFS): g_refs holds each stack's handle instead; the member's own record (g_recs) gives the offset.
-template <bool MERGED, bool REFS = false, bool HANDLES = false>
+// REFS (with MERGED): frames come from the member's registered arena; the gathered handle (g_refs) names the member's own record
+// (g_recs), which gives the offset.
+template <bool MERGED, bool REFS = false>
 __global__ void __launch_bounds__(kThreads) k_store_insert(StoreInsertArgs a) {
   const unsigned full = 0xFFFFFFFFu;
   uint32_t nu = a.ctr->n_unique;
@@ -2493,16 +2495,14 @@ __global__ void __launch_bounds__(kThreads) k_store_insert(StoreInsertArgs a) {
         continue;
       }
       unsigned long long base = size ? a.g_refs[k] : 0ull;
-      if constexpr (HANDLES) {
-        if (size) {  // the sender's k_header accepted this handle in this batch, so a mismatch here is a logic error
-          const uint32_t slot = (uint32_t)base, gen = (uint32_t)(base >> 32);
-          const uint4 s1 = slot < a.n_recs ? __ldg(a.g_recs + 2ull * slot + 1) : make_uint4(0u, 0u, 0u, kStackFree);
-          if (s1.w != gen || (gen & kStackFree) || s1.z != size) {
-            if (lane == 0) atomicOr(&a.ctr_w->err, ERR_MERGE_LOOKUP);
-            continue;
-          }
-          base = ((unsigned long long)s1.y << 32) | s1.x;
+      if (size) {  // the sender's k_header accepted this handle in this batch, so a mismatch here is a logic error
+        const uint32_t slot = (uint32_t)base, gen = (uint32_t)(base >> 32);
+        const uint4 s1 = slot < a.n_recs ? __ldg(a.g_recs + 2ull * slot + 1) : make_uint4(0u, 0u, 0u, kStackFree);
+        if (s1.w != gen || (gen & kStackFree) || s1.z != size) {
+          if (lane == 0) atomicOr(&a.ctr_w->err, ERR_MERGE_LOOKUP);
+          continue;
         }
+        base = ((unsigned long long)s1.y << 32) | s1.x;
       }
       for (uint32_t j = lane; j < size; j += 32) {
         unsigned long long fid = frame_at(a.frames, base + j, a.narrow);
@@ -3079,9 +3079,9 @@ __global__ void __launch_bounds__(kThreads) k_store_pack(const MergeCtl* mc, con
     }
   }
 }
-// PA_CFG_GROUP_STACKS groups: every member holds the same registered arena, so a stack the store lacks crosses as one reference
-// instead of its frames — the arena offset of its global first occurrence (the row's frame_off after k_header<true>), which
-// keeps that occurrence's frames when two registered stacks share a provided id
+// PA_CFG_GROUP_STACKS groups: every member holds the same registered stacks, so a stack the store lacks crosses as one reference
+// instead of its frames — the handle of its global first occurrence, which keeps that occurrence's frames when two registered
+// stacks share a provided id
 struct StoreRefsF {  // where each merged stack's reference goes in the gathered buffer: exclusive scan of (k_store_need != 0)
   typedef unsigned long long T;
   const Counters* ctr;
@@ -3092,16 +3092,14 @@ struct StoreRefsF {  // where each merged stack's reference goes in the gathered
   __device__ void emit(uint32_t u, unsigned long long ex, unsigned long long) const { ridx[u] = ex; }
   __device__ void total(int, unsigned long long t) const { ridx[ctr->n_unique] = t; }
 };
-// this shard's block: the references of its won stacks that k_store_need selected. A row's reference is ref[row * ref_stride]:
-// its frame_off after k_header (stride 1), or, in PA_CFG_GROUP_RETIRE groups, the handle its header still carries (the
-// pa_sample_hdr's frame_off word, stride 8)
+// this shard's block: the references of its won stacks that k_store_need selected. A row's reference is the handle its header
+// still carries: hdr_foff points at row 0's frame_off word, and the 64-byte headers are 8 words apart
 __global__ void __launch_bounds__(kThreads) k_store_pack_refs(const MergeCtl* mc, const uint32_t* g_row, uint32_t row_base, const uint32_t* need,
-                                                              const unsigned long long* ridx, const unsigned long long* ref, uint32_t ref_stride,
-                                                              unsigned long long* out) {
+                                                              const unsigned long long* ridx, const unsigned long long* hdr_foff, unsigned long long* out) {
   const uint32_t o0 = mc->ord0, o1 = mc->ord1;
   const unsigned long long base0 = ridx[o0];
   for (uint32_t u = o0 + blockIdx.x * kThreads + threadIdx.x; u < o1; u += gridDim.x * kThreads)
-    if (need[u]) out[ridx[u] - base0] = ref[(size_t)(g_row[u] - row_base) * ref_stride];
+    if (need[u]) out[ridx[u] - base0] = hdr_foff[(size_t)(g_row[u] - row_base) * 8];
 }
 
 // ---------------------------------------------------------------------------------------------

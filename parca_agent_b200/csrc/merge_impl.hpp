@@ -835,7 +835,7 @@ static int merge_process_once(pa_merge* g, bool* retry) {
 // (all-gather-v; near zero in steady state). Every decision below depends only on replicated state, so every rank takes it.
 
 // the frames the insert may need (k_store_need on the store as it is now), gathered into every member's v1_frames; in
-// PA_CFG_GROUP_STACKS groups one arena offset per such stack instead (v1_foff then indexes references, not frames)
+// PA_CFG_GROUP_STACKS groups one handle per such stack instead (v1_foff then indexes references, not frames)
 static int store_frames_exchange(pa_merge* g, uint32_t min_last_p1) {
   const size_t L = g->members.size();
   const uint32_t W = g->world;
@@ -877,11 +877,10 @@ static int store_frames_exchange(pa_merge* g, uint32_t min_last_p1) {
     MCK(mb.v1_send.ensure(std::max<uint64_t>(count[me], 256)));
     MCK(mb.v1_frames.ensure(std::max<uint64_t>(b[W] * unit, 256)));
     if (refs) {
-      // group retire: the handle (the header's frame_off word), since the members' arenas may differ in layout
-      const unsigned long long* ref = g->group_retire ? a->d_hdr.as<unsigned long long>() + offsetof(pa_sample_hdr, frame_off) / 8 : a->d_foff.as<unsigned long long>();
+      static_assert(sizeof(pa_sample_hdr) == 64, "k_store_pack_refs reads the handles 8 words apart");
       k_store_pack_refs<<<small_grid(a, U), kThreads, 0, a->s_comp>>>((const MergeCtl*)(mb.ctl.as<uint32_t>() + CTL_MERGE), mb.g_uniq_row.as<uint32_t>(),
                                                                       (uint32_t)g->row_base[me], mb.v1_need.as<uint32_t>(), mb.v1_foff.as<unsigned long long>(),
-                                                                      ref, g->group_retire ? (uint32_t)(sizeof(pa_sample_hdr) / 8) : 1u,
+                                                                      a->d_hdr.as<unsigned long long>() + offsetof(pa_sample_hdr, frame_off) / 8,
                                                                       mb.v1_send.as<unsigned long long>());
       a->store_refs_sent += count[me] / 8;
       src[i] = mb.v1_send.p; dst[i] = mb.v1_frames.p;
@@ -950,11 +949,10 @@ static int merge_store_update(pa_merge* g) {
       StoreInsertArgs sa = store_insert_args(a, min_last_p1);
       sa.gtab = mb.gtab.as<StackSlot>(); sa.g_slot = mb.g_uniq_slot.as<uint32_t>(); sa.g_last_inv = last[i];
       sa.g_frames = mb.v1_frames.as<uint32_t>(); sa.g_foff = mb.v1_foff.as<unsigned long long>();
-      if (g->group_retire) {
+      if (g->group_stacks) {
         sa.g_refs = mb.v1_frames.as<unsigned long long>(); sa.g_recs = (const uint4*)a->d_rs_recs.p; sa.n_recs = a->P.n_stacks;
-        k_store_insert<true, true, true><<<a->G, kThreads, 0, a->s_comp>>>(sa);
-      } else if (g->group_stacks) { sa.g_refs = mb.v1_frames.as<unsigned long long>(); k_store_insert<true, true><<<a->G, kThreads, 0, a->s_comp>>>(sa); }
-      else k_store_insert<true><<<a->G, kThreads, 0, a->s_comp>>>(sa);
+        k_store_insert<true, true><<<a->G, kThreads, 0, a->s_comp>>>(sa);
+      } else k_store_insert<true><<<a->G, kThreads, 0, a->s_comp>>>(sa);
       MCK(cudaMemcpyAsync(a->h_ctr_pinned, ctr, sizeof(Counters), cudaMemcpyDeviceToHost, a->s_comp));
       if ((rc = store_ctl_read(a, &ctl))) return g->fail(rc, a->err);
       MCK(cudaGetLastError());
@@ -1020,7 +1018,7 @@ static int merge_process(pa_merge* g) {
   StreamShare share(g);
   auto restore = [] {};
   // ---- rows of every shard -> global row ranges; registrations must be identical (ids are global)
-  // (group retire: n_stack_frames is the frames of the stacks not yet freed, since dead frames make arena lengths differ)
+  // (group stacks: n_stack_frames is the frames of the stacks not yet freed, since dead frames make arena lengths differ)
   struct Dims { uint64_t n, nf, store_entries, store_frames, n_stack_frames, stack_digest, stages;
                 uint32_t ncols, nlab, n_frames, n_cstr, n_labelsets, n_funcs, lz4, schema, group_stacks, n_stacks, group_retire; };
   std::vector<const void*> src(L);
@@ -1029,7 +1027,7 @@ static int merge_process(pa_merge* g) {
   for (size_t i = 0; i < L && !rc; i++) {
     pa_agg* a = g->members[i];
     cudaSetDevice(a->device);
-    Dims d{a->N, a->NF, a->store_entries, a->store_frames, a->group_retire ? a->P.stack_frames_live : a->P.n_stack_frames, a->P.stack_digest,
+    Dims d{a->N, a->NF, a->store_entries, a->store_frames, a->P.stack_frames_live, a->P.stack_digest,
            a->group_retire ? a->rs_stages : 0, (uint32_t)a->cols.size(), a->n_label_cols, a->P.n_frames, a->P.n_cstr, a->P.n_labelsets, a->P.n_funcs,
            g->lz4 ? 1u : 0u, (uint32_t)a->cfg.schema, a->group_stacks ? 1u : 0u, a->P.n_stacks, a->group_retire ? 1u : 0u};
     if (g->mb[i].gather_scratch.ensure(std::max<size_t>((size_t)(W + 1) * sizeof(Dims), 256)) != cudaSuccess) { rc = g->fail(PA_ENOMEM, "device allocation failed"); break; }
@@ -1074,8 +1072,7 @@ static int merge_process(pa_merge* g) {
   }
   g->row_base[W] = g->NT;
   // group stacks: the rings hold no frames; the merged location-index stream, and each shard's slice of it, is bounded by the
-  // (identical) registered arena, as one registered-stacks aggregator's is; with group retire by the frames of the stacks not yet
-  // freed, which every stack a row may name belongs to
+  // frames of the (identical) registered stacks not yet freed, which every stack a row may name belongs to
   if (g->group_stacks) g->NFT = dims[0].n_stack_frames;
   g->ncols = dims[0].ncols;
   if (g->NT > 0x7FFFFFFFull) { restore(); return g->fail(PA_ERANGE, "merged batch exceeds the int32 row limit of run ends / ListView offsets"); }

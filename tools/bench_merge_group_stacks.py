@@ -6,7 +6,7 @@ one GPU. Config-4 shards of --rows rows each (pid-sharded parts of one 8-GPU con
       at create, and after the warm-up flush, which adds the device mirrors of the registered tables (the registered stacks'
       records and arena among them), the per-flush scratch and the group's exchange buffers;
   (b) the same shards as v1 groups: the bytes of the store exchange in the cold first interval (4 B per frame id for the ring
-      group, one 8-byte arena offset per stack for the group-stacks group) and in a repeat of it;
+      group, one 8-byte handle per stack for the group-stacks group) and in a repeat of it;
   (c) all 8 shards of the interval (8 x --rows rows, which a ring group cannot hold on one 80 GB card) as ONE group-stacks group,
       built member by member until the card is full; then the group is freed and one group-stacks aggregator takes the
       concatenated rows of the shards that fitted: its sha256 must equal the group's.
