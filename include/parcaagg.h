@@ -301,7 +301,11 @@ int pa_agg_collect(pa_agg* a, pa_agg_result* out);
 /* device time (ms, CUDA events on the compute stream) of named kernel groups during the last
  * process(): names are "hash", "header", "rank", "locations", "labels", "dicts", "total". "lz4" reports the compression kernels of
  * the last collect / pa_agg_stacktraces in PA_IPC_LZ4_FRAME_GPU mode. Two more names report counters of the
- * v1 stack store since creation in *launches (ms = 0): "store_compactions", "store_evictions". */
+ * v1 stack store since creation in *launches (ms = 0): "store_compactions", "store_evictions". Two more report the label
+ * column plan in *launches (ms = 0): "label_columns", the labelset-derived label columns planned for the last pass (a pass plans
+ * the label names the previous batch's rows used plus every name registered since; at most 246 label columns, cpu / thread_id /
+ * thread_name included, per batch), and "label_replans", the passes redone since creation because a batch's rows used a
+ * label name the plan had left out. */
 int pa_agg_last_kernel_ms(const pa_agg* a, const char* name, double* ms, uint32_t* launches);
 /* copies the per-row 128-bit stack ids (big-endian hi‖lo, 16 B per row) of the staged batch. */
 int pa_agg_debug_stack_ids(pa_agg* a, uint8_t* out, uint64_t n_rows);

@@ -76,9 +76,8 @@ struct Mirror {
 struct ColPlan {
   std::string name;
   uint32_t type = COL_LS;
-  uint32_t param = 0;              // LS: column index in lsmat; KIND: table row
-  std::vector<uint32_t> vals;      // LS: local value id -> canonical string id
-  std::map<uint32_t, uint32_t> val_index;
+  uint32_t param = 0;              // LS: column of the batch's key matrix; KIND: table row
+  uint32_t ord = 0;                // LS: the label name's ordinal (its value ids index LabelSets::vals[ord])
   uint32_t universe = 0;
   // device pointers for this flush
   int* run_ends = nullptr;
@@ -105,8 +104,8 @@ struct MergeDims { uint32_t world = 1, rank = 0; uint64_t row_base = 0, n_total 
 // everything the stages of one pass share (valid from pass_plan until the batch is collected)
 struct Pass {
   // registration state as mirrored to the device for this batch (snapshot taken under reg_mu in upload_tables)
-  uint32_t n_cstr = 0, n_frames = 0, n_funcs = 0, n_sids = 0, n_labelsets = 0;
-  uint32_t n_stacks = 0;          // stack slots on the device (PA_CFG_REGISTERED_STACKS)
+  uint32_t n_cstr = 0, n_frames = 0, n_funcs = 0, n_sids = 0, n_labelsets = 0, n_names = 0;
+  uint32_t n_stacks = 0;         // stack slots on the device (PA_CFG_REGISTERED_STACKS)
   uint64_t n_stack_frames = 0;    // and the frame ids of their arena (freed stacks' included until a compaction)
   uint64_t stack_digest = 0;      // PA_CFG_GROUP_STACKS: digest of those stacks (merge groups check it is the same on every member)
   uint64_t stack_frames_live = 0; // frames of the uploaded stacks not yet freed (in a merge group, the same on every member)
@@ -120,7 +119,10 @@ struct Pass {
   uint32_t *rowbits = nullptr, *row_wprefix = nullptr, *uniq_slot = nullptr, *uniq_size = nullptr, *first_ls = nullptr, *claimed = nullptr;
   uint32_t *loc_bits = nullptr, *loc_wp = nullptr, *sd_bits[4] = {}, *sd_wp[4] = {}, *fn_bits = nullptr, *fn_wp = nullptr;
   unsigned long long* edge_keys = nullptr;
-  uint32_t* red_block = nullptr;  // [first_ls | first_cpu | first_comm | v1: first_kind]: the direct first-row tables mode B all-reduces
+  // label column plan check (k_ls_plan): per labelset its row of the key matrix [used labelsets][planned LS columns], the
+  // used-labelset count, the used-name bitmap over the name ordinals (read back with the counters)
+  uint32_t *ls_rank = nullptr, *ls_keys = nullptr, *ls_used = nullptr, *used_names = nullptr;
+  uint32_t* red_block = nullptr; // [first_ls | first_cpu | first_comm | v1: first_kind]: the direct first-row tables mode B all-reduces
   size_t red_count = 0;
   std::vector<uint32_t*> col_first, col_rank, col_bits, col_wp;
   int j_loc = 0, j_type = 0, j_file = 0, j_lab0 = 0;
@@ -173,10 +175,17 @@ struct pa_agg {
   FrameTableHost ft;
   LabelSets ls;
   std::vector<std::pair<uint32_t, uint32_t>> external;  // canonical ids
-  bool cols_dirty = true;
-  std::vector<ColPlan> cols;  // label columns, then the 8 constant-ish columns
-  uint32_t n_label_cols = 0, n_lscols = 0;
-  std::vector<uint32_t> lsmat;
+  std::vector<ColPlan> cols;  // label columns of this batch's plan, then the 8 constant-ish columns
+  uint32_t n_label_cols = 0, n_lscols = 0;  // label columns; the labelset-derived ones among them (the first n_lscols)
+  // Label column plan (DESIGN section 4): the labelset-derived columns of a batch are a predicted set of name ordinals, the
+  // names the previous batch's rows used plus every name registered since; the pass checks it and is redone on a miss.
+  std::vector<uint32_t> used_prev;  // name ordinals the rows of the last processed batch used, ascending
+  uint32_t names_planned = 0;       // names registered when that batch was planned
+  bool plan_pending = false;        // a batch was planned and has not completed: the next plan starts cold
+  uint64_t label_replans = 0;       // passes redone because the prediction missed a used name, since creation
+  uint64_t plan_digest = 0;         // digest of the planned name ordinals (merge groups check that every member has the same plan)
+  uint32_t* h_used = nullptr;       // pinned: the used-name bitmap of the last pass
+  size_t h_used_words = 0;
   std::vector<uint32_t> kindtab;           // [8][8]
   std::vector<std::vector<std::string>> kind_strings;  // class -> string for the 6 string columns
   std::vector<int64_t> period_vals;
@@ -184,7 +193,8 @@ struct pa_agg {
 
   Mirror<uint64_t> m_addr, m_line;
   Mirror<uint32_t> m_type, m_map, m_bid, m_func, m_fnfile, m_sid2cid;
-  DBuf d_lsmat, d_kindtab, d_cols, d_jobs;
+  Mirror<uint32_t> m_ls_off, m_ls_pairs;  // the registered labelsets (LabelSets::off, LabelSets::pairs)
+  DBuf d_kindtab, d_cols, d_jobs;
   // PA_CFG_REGISTERED_STACKS: the stack registry. The device holds it (records, last_use, the frame arena with ids at the ring's
   // width, idb / 4 words each). The host keeps per-slot metadata, the free slots (a min-heap), the retired stacks waiting for
   // their grace batch, and the registrations not yet uploaded. Without PA_CFG_RETIRE_STACKS no slot is ever freed, so every
@@ -350,54 +360,87 @@ static void build_kind_tables(pa_agg* a) {
   }
 }
 
-static int build_columns(pa_agg* a) {
+// cpu / thread_id / thread_name columns of the config; a labelset's pair of the same name never reaches a column when the
+// column is on: the per-sample labels.Builder.Set overrides the cached value (:616-625)
+static uint32_t sample_label_cols(const pa_agg* a) {
+  const uint32_t f = a->cfg.label_flags;
+  return !(f & PA_LABEL_DISABLE_CPU) + !(f & PA_LABEL_DISABLE_THREAD_ID) + !(f & PA_LABEL_DISABLE_THREAD_COMM);
+}
+static bool overridden_name(const pa_agg* a, uint32_t name_cid) {
+  const uint32_t f = a->cfg.label_flags, n = a->sp.len(name_cid);
+  const char* p = (const char*)a->sp.ptr(name_cid);
+  auto is = [&](const char* z) { return n == strlen(z) && !memcmp(p, z, n); };
+  return (is("cpu") && !(f & PA_LABEL_DISABLE_CPU)) || (is("thread_id") && !(f & PA_LABEL_DISABLE_THREAD_ID)) ||
+         (is("thread_name") && !(f & PA_LABEL_DISABLE_THREAD_COMM));
+}
+// the label columns take kMaxCols minus the 8 kind-derived columns and v1's two
+static bool plan_fits(const pa_agg* a, size_t n_names) { return n_names + sample_label_cols(a) + 10 <= (size_t)kMaxCols; }
+
+// The column plan of a batch: one labelset-derived column per planned name ordinal (ascending), the sample label columns,
+// the kind-derived columns. reg_mu held.
+static int build_columns(pa_agg* a, const std::vector<uint32_t>& names) {
+  if (!plan_fits(a, names.size())) return a->fail(PA_ERANGE, "too many distinct label names in one batch (limit 246)");
   a->cols.clear();
   const uint32_t flags = a->cfg.label_flags;
-  const bool on_cpu = !(flags & PA_LABEL_DISABLE_CPU), on_tid = !(flags & PA_LABEL_DISABLE_THREAD_ID), on_comm = !(flags & PA_LABEL_DISABLE_THREAD_COMM);
-  const uint32_t c_cpu = a->sp.intern("cpu"), c_tid = a->sp.intern("thread_id"), c_comm = a->sp.intern("thread_name");
-  std::map<uint32_t, uint32_t> col_of_name;  // name cid -> column
-  a->n_lscols = 0;
-  for (auto& set : a->ls.sets)
-    for (auto& kv : set) {
-      uint32_t name = kv.first;
-      // per-sample labels.Builder.Set overrides the cached value of the same name (:616-625)
-      if ((name == c_cpu && on_cpu) || (name == c_tid && on_tid) || (name == c_comm && on_comm)) continue;
-      auto it = col_of_name.find(name);
-      if (it == col_of_name.end()) {
-        ColPlan c;
-        c.name.assign((const char*)a->sp.ptr(name), a->sp.len(name));
-        c.type = COL_LS;
-        c.param = a->n_lscols++;
-        it = col_of_name.emplace(name, (uint32_t)a->cols.size()).first;
-        a->cols.push_back(std::move(c));
-      }
-      ColPlan& c = a->cols[it->second];
-      if (!c.val_index.count(kv.second)) { c.val_index.emplace(kv.second, (uint32_t)c.vals.size()); c.vals.push_back(kv.second); }
-    }
-  a->lsmat.assign((size_t)std::max<size_t>(1, a->ls.sets.size()) * std::max<uint32_t>(1, a->n_lscols), kNull);
-  for (size_t s = 0; s < a->ls.sets.size(); s++)
-    for (auto& kv : a->ls.sets[s]) {
-      auto it = col_of_name.find(kv.first);
-      if (it == col_of_name.end()) continue;
-      ColPlan& c = a->cols[it->second];
-      a->lsmat[s * std::max<uint32_t>(1, a->n_lscols) + c.param] = c.val_index[kv.second];
-    }
-  for (auto& c : a->cols) c.universe = (uint32_t)c.vals.size();
+  for (uint32_t ord : names) {
+    ColPlan c;
+    const uint32_t cid = a->ls.name_cid[ord];
+    c.name.assign((const char*)a->sp.ptr(cid), a->sp.len(cid));
+    c.type = COL_LS;
+    c.param = (uint32_t)a->cols.size();
+    c.ord = ord;
+    c.universe = (uint32_t)a->ls.vals[ord].size();
+    a->cols.push_back(std::move(c));
+  }
+  a->n_lscols = (uint32_t)a->cols.size();
+  uint64_t d = 0xcbf29ce484222325ull ^ names.size();  // FNV-1a over the ordinals
+  for (uint32_t ord : names) d = (d ^ ord) * 0x100000001b3ull;
+  a->plan_digest = d;
   auto add = [a](const char* name, uint32_t type, uint32_t universe) { ColPlan c; c.name = name; c.type = type; c.universe = universe; a->cols.push_back(std::move(c)); };
-  if (on_cpu) add("cpu", COL_CPU, 65536);
-  if (on_tid) add("thread_id", COL_TID, 0);
-  if (on_comm) add("thread_name", COL_COMM, 0 /* = canonical string count, set per flush */);
+  if (!(flags & PA_LABEL_DISABLE_CPU)) add("cpu", COL_CPU, 65536);
+  if (!(flags & PA_LABEL_DISABLE_THREAD_ID)) add("thread_id", COL_TID, 0);
+  if (!(flags & PA_LABEL_DISABLE_THREAD_COMM)) add("thread_name", COL_COMM, 0 /* = canonical string count, set per flush */);
   a->n_label_cols = (uint32_t)a->cols.size();
-  if (a->n_label_cols + 10 > (uint32_t)kMaxCols) return a->fail(PA_ERANGE, "too many distinct label names (limit 246)");
   static const char* fixed[8] = {"producer", "sample_type", "sample_unit", "period_type", "period_unit", "temporality", "period", "duration"};
   for (uint32_t t = 0; t < 8; t++) { ColPlan c; c.name = fixed[t]; c.type = COL_KIND; c.param = t; a->cols.push_back(std::move(c)); }
   if (a->cfg.schema == PA_SCHEMA_V1) {  // v1: stacktrace_id and timestamp are run-end encoded too (arrow.go:395-400, :471-474)
     ColPlan o; o.name = "stacktrace_id"; o.type = COL_ORD; a->cols.push_back(std::move(o));
     ColPlan t; t.name = "timestamp"; t.type = COL_TS; a->cols.push_back(std::move(t));
   }
-  build_kind_tables(a);
-  a->cols_dirty = false;
   return PA_OK;
+}
+
+// The predicted plan (reg_mu held, P.n_names snapshotted): the names the previous batch's rows used plus every name registered
+// since it was planned; when that does not fit, the previously used names alone; when those do not either, none. A cold
+// start (no previous batch, or the previous one failed) has no used names and every name is new. The pass checks the
+// prediction on the device and is redone with exactly the used names when it missed one (replan_labels).
+static int plan_labels(pa_agg* a) {
+  if (a->plan_pending) { a->used_prev.clear(); a->names_planned = 0; }
+  std::vector<uint32_t> pred = a->used_prev;
+  for (uint32_t o = a->names_planned; o < a->P.n_names; o++) pred.push_back(o);  // (every used ordinal is below names_planned)
+  if (!plan_fits(a, pred.size())) pred = plan_fits(a, a->used_prev.size()) ? a->used_prev : std::vector<uint32_t>{};
+  a->plan_pending = true;
+  return build_columns(a, pred);
+}
+// The members of a merge group predicted different plans (one of them flushed alone since the last merged batch): every member
+// plans cold, which depends on the registrations only, so the columns are the same on every member again (reg_mu not held)
+static int plan_cold(pa_agg* a) {
+  std::lock_guard<std::mutex> g(a->reg_mu);
+  a->plan_pending = true;  // plan_labels then starts from no used names and the first name
+  return plan_labels(a);
+}
+// the names the last pass's rows used, from the bitmap pass_finish read back
+static std::vector<uint32_t> used_names(const pa_agg* a) {
+  std::vector<uint32_t> v;
+  for (uint32_t w = 0; w < (a->P.n_names + 31) / 32; w++)
+    for (uint32_t m = a->h_used[w]; m; m &= m - 1) v.push_back(w * 32 + (uint32_t)__builtin_ctz(m));
+  return v;
+}
+// the prediction missed a name: plan exactly the used ones for the redo
+static int replan_labels(pa_agg* a) {
+  std::lock_guard<std::mutex> g(a->reg_mu);
+  a->label_replans++;
+  return build_columns(a, used_names(a));
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -554,10 +597,11 @@ void pa_agg_destroy(pa_agg* a) {
   if (a->h_ctr_pinned) cudaFreeHost(a->h_ctr_pinned);
   if (a->out) cudaFreeHost(a->out);
   if (a->h_desc) cudaFreeHost(a->h_desc);
+  if (a->h_used) cudaFreeHost(a->h_used);
   DBuf* all[] = {&a->d_hdr, &a->d_frames, &a->d_ts, &a->d_value, &a->d_uuid, &a->d_stoff, &a->d_stsize, &a->d_slot, &a->d_kind, &a->d_nfr,
                  &a->d_foff, &a->d_ls, &a->d_cpu, &a->d_tid, &a->d_comm, &a->d_ustream, &a->d_uniq_row, &a->d_uniq_count, &a->d_table, &a->d_ctr,
-                 &a->d_arena, &a->d_partial, &a->d_partial2, &a->d_ree_partial, &a->d_lsmat, &a->d_kindtab, &a->d_cols, &a->d_jobs,
-                 &a->m_addr.buf, &a->m_line.buf, &a->m_type.buf, &a->m_map.buf, &a->m_bid.buf, &a->m_func.buf, &a->m_fnfile.buf, &a->m_sid2cid.buf,
+                 &a->d_arena, &a->d_partial, &a->d_partial2, &a->d_ree_partial, &a->d_kindtab, &a->d_cols, &a->d_jobs,
+                 &a->m_addr.buf, &a->m_line.buf, &a->m_type.buf, &a->m_map.buf, &a->m_bid.buf, &a->m_func.buf, &a->m_fnfile.buf, &a->m_sid2cid.buf, &a->m_ls_off.buf, &a->m_ls_pairs.buf,
                  &a->m1_map.buf, &a->m1_bid.buf, &a->m1_fn.buf, &a->m1_file.buf, &a->m1_line.buf, &a->m1_col.buf, &a->m1_complete.buf,
                  &a->d_store, &a->d_store_arena, &a->d_store_ctl, &a->d_v1_ids, &a->d_st1, &a->d_store_stamp, &a->d_v1_last, &a->d_select, &a->d_lz4, &a->d_lz4_body,
                  &a->d_rs_recs, &a->d_rs_last, &a->d_rs_arena[0], &a->d_rs_arena[1], &a->d_rs_tmp, &a->d_rs_upd};
@@ -604,18 +648,18 @@ int pa_agg_register_frames(pa_agg* a, const pa_frame_desc* descs, uint32_t n, ui
 int pa_agg_register_labelsets(pa_agg* a, const pa_label_pair* pairs, const uint32_t* offsets, uint32_t n, uint32_t* first_id) {
   if (!a || (n && !offsets)) return PA_EINVAL;
   std::lock_guard<std::mutex> g(a->reg_mu);
-  if (first_id) *first_id = (uint32_t)a->ls.sets.size();
+  if (first_id) *first_id = a->ls.count();
   for (uint32_t i = 0; i < n; i++) {
     std::vector<std::pair<uint32_t, uint32_t>> set;
     for (uint32_t k = offsets[i]; k < offsets[i + 1]; k++) {
       if (pairs[k].name_sid >= a->sp.sid2cid.size() || pairs[k].value_sid >= a->sp.sid2cid.size()) return a->fail(PA_EINVAL, "labelset refers to an unregistered string id");
-      uint32_t v = a->sp.sid2cid[pairs[k].value_sid];
+      uint32_t v = a->sp.sid2cid[pairs[k].value_sid], name = a->sp.sid2cid[pairs[k].name_sid];
       if (v == 0) continue;  // labels.Labels never carries empty values
-      set.emplace_back(a->sp.sid2cid[pairs[k].name_sid], v);
+      if (overridden_name(a, name)) continue;
+      set.emplace_back(name, v);
     }
-    a->ls.sets.push_back(std::move(set));
+    a->ls.add(set);
   }
-  a->cols_dirty = true;
   return PA_OK;
 }
 // Validation shared by both registration calls (a refused call registers nothing). check_stack_args runs before reg_mu is
@@ -999,7 +1043,8 @@ static int rs_stage(pa_agg* a) {
   return rs_upload(a, frees, slots, true);
 }
 
-static int upload_tables(pa_agg* a) {
+// plan_batch: a pass follows, which takes the label column plan predicted here (pa_agg_stacktraces only needs the mirrors)
+static int upload_tables(pa_agg* a, bool plan_batch) {
   std::lock_guard<std::mutex> g(a->reg_mu);
   cudaStream_t s = a->s_comp;
   CK(a->m_addr.sync(a->ft.addr, s)); CK(a->m_line.sync(a->ft.line, s)); CK(a->m_type.sync(a->ft.type_cid, s));
@@ -1014,20 +1059,16 @@ static int upload_tables(pa_agg* a) {
     int rc = rs_upload(a, {}, {}, false);
     if (rc) return rc;
   }
+  CK(a->m_ls_off.sync(a->ls.off, s)); CK(a->m_ls_pairs.sync(a->ls.pairs, s));
   // what the device mirrors now hold: the pass uses these counts only (registration may continue concurrently)
   a->P.n_cstr = a->sp.count(); a->P.n_frames = a->ft.count(); a->P.n_funcs = a->ft.n_funcs();
-  a->P.n_sids = (uint32_t)a->sp.sid2cid.size(); a->P.n_labelsets = (uint32_t)a->ls.sets.size();
-  if (a->cols_dirty) {
-    int rc = build_columns(a);
-    if (rc) return rc;
-    a->P.n_cstr = a->sp.count();  // the column plan may intern label names
-    CK(a->d_lsmat.ensure(a->lsmat.size() * 4));
-    CK(cudaMemcpyAsync(a->d_lsmat.p, a->lsmat.data(), a->lsmat.size() * 4, cudaMemcpyHostToDevice, s));
+  a->P.n_sids = (uint32_t)a->sp.sid2cid.size(); a->P.n_labelsets = a->ls.count(); a->P.n_names = a->ls.n_names();
+  if (!a->d_kindtab.p) {
+    build_kind_tables(a);
     CK(a->d_kindtab.ensure(a->kindtab.size() * 4));
     CK(cudaMemcpyAsync(a->d_kindtab.p, a->kindtab.data(), a->kindtab.size() * 4, cudaMemcpyHostToDevice, s));
-    CK(cudaStreamSynchronize(s));  // lsmat/kindtab host vectors may be rebuilt later
   }
-  return PA_OK;
+  return plan_batch ? plan_labels(a) : PA_OK;
 }
 
 // first-occurrence ranking of a batch of FoJobs (blockIdx.y = job). elem_bound: upper bound on elements per job;
@@ -1259,6 +1300,21 @@ static int pass_plan(pa_agg* a, const MergeDims* md) {
   if (v1) want(&a->v1_first_kind, 8 * 4, 0);  // (a merged batch takes the minimum over the shards: the kind columns' dictionary order)
   size_t red_bytes = 0;
   for (auto& r : reqs) red_bytes += r.bytes;
+  // the label column plan check: the key matrix has one row per labelset the (merged) batch names, at most one per row
+  P.ls_rank = P.ls_keys = P.ls_used = P.used_names = nullptr;
+  if (P.n_names) {
+    const size_t used_words = (P.n_names + 31) / 32;
+    want(&P.ls_rank, (size_t)P.n_labelsets * 4);
+    want(&P.ls_keys, std::max<size_t>((size_t)std::min<uint64_t>(P.n_labelsets, NTn) * a->n_lscols, 1) * 4);
+    want(&P.ls_used, 4, 1); want(&P.used_names, used_words * 4, 1);
+    if (used_words > a->h_used_words) {
+      if (a->h_used) cudaFreeHost(a->h_used);
+      a->h_used = nullptr;
+      a->h_used_words = 0;
+      CK(cudaHostAlloc((void**)&a->h_used, used_words * 2 * 4, cudaHostAllocDefault));
+      a->h_used_words = used_words * 2;
+    }
+  }
   if (v1) {
     want(&a->v1_ord, Nn * 4); want(&a->v1_ts_vals, Nn * 8); want(&a->v1_id_off, (Nn + 1) * 4);
     a->v1_ids = a->d_v1_ids.as<uint8_t>();  // outlives the arena: pa_agg_last_stack_ids / pa_agg_stacktraces run after the flush
@@ -1348,7 +1404,7 @@ static int pass_plan(pa_agg* a, const MergeDims* md) {
   for (uint32_t c = 0; c < nlab; c++) {
     ColPlan& cp = a->cols[c];
     bool nullable = cp.type == COL_LS || cp.type == COL_COMM;
-    // first ROWS are recorded by k_header / k_ls_first (skip_min); the emit pass applies the ranks itself (no map pass)
+    // first ROWS are recorded by k_header / k_ls_plan (skip_min); the emit pass applies the ranks itself (no map pass)
     int ji = job(nullptr, nullptr, P.col_first[c], cp.universe, P.col_rank[c], cp.order, nullptr, nullptr, P.col_bits[c], P.col_wp[c],
                  &ctr->n_dict[c], nullptr, nullable, true);
     jobs[ji].n_imm = (uint32_t)P.NT;
@@ -1374,7 +1430,7 @@ static int pass_plan(pa_agg* a, const MergeDims* md) {
   if (v1) { ra.ord = a->v1_ord; ra.ts = a->d_ts.as<long long>(); ra.ts_vals = a->v1_ts_vals; ra.kindrank = a->v1_kindrank; ra.kind_dict_mask = 0x3Fu; }
   ra.n_rows = (uint32_t)N; ra.ncols = ncols; ra.n_ls = a->n_lscols; ra.c_kind = nlab; ra.cols = nullptr /* set after the upload */;
   ra.ls = a->d_ls.as<uint32_t>(); ra.cpu = a->d_cpu.as<uint32_t>(); ra.tid = a->d_tid.as<uint32_t>(); ra.comm = a->d_comm.as<uint32_t>(); ra.kind = a->d_kind.as<uint8_t>();
-  ra.lsmat = a->d_lsmat.as<uint32_t>(); ra.n_lscols = std::max<uint32_t>(1, a->n_lscols); ra.kindtab = a->d_kindtab.as<uint32_t>();
+  ra.ls_rank = P.ls_rank; ra.ls_keys = P.ls_keys; ra.n_lscols = std::max<uint32_t>(1, a->n_lscols); ra.kindtab = a->d_kindtab.as<uint32_t>();
   ra.partial = a->d_ree_partial.as<uint32_t>(); ra.ctr = ctr;
   ra.row_base = (uint32_t)P.row_base; ra.edge_keys = md ? P.edge_keys : nullptr; ra.mc = nullptr;
   ReeGroups& rg = P.rg;  // one launch row per column (the 8 kind-derived columns form one group)
@@ -1422,7 +1478,7 @@ static int pass_front(pa_agg* a) {
     h.ls = a->d_ls.as<uint32_t>(); h.cpu = a->d_cpu.as<uint32_t>(); h.tid = a->d_tid.as<uint32_t>(); h.comm = a->d_comm.as<uint32_t>();
     h.sid2cid = a->m_sid2cid.ptr(); h.n_sids = P.n_sids; h.n_labelsets = P.n_labelsets;
     h.n_frame_ids = frames_end; h.provided = provided ? 1 : 0; h.tab = tab; h.mask = P.mask; h.slot_of_row = a->d_slot.as<uint32_t>(); h.ctr = ctr; h.claimed = P.claimed;
-    h.first_ls = a->n_lscols ? P.first_ls : nullptr;
+    h.first_ls = P.n_names ? P.first_ls : nullptr;
     for (uint32_t c = 0; c < P.nlab; c++) {
       if (a->cols[c].type == COL_CPU) h.first_cpu = P.col_first[c];
       if (a->cols[c].type == COL_TID) { h.tid_slots = a->tid_slots; h.tid_mask = a->tid_mask; }
@@ -1576,12 +1632,14 @@ static int pass_labels_count(pa_agg* a, cudaStream_t s) {
   Pass& P = a->P;
   if (getenv("PA_DEBUG_SYNC")) CK(cudaStreamSynchronize(s));
   CK(cudaEventRecord(a->tm[T_LABELS].a, s));
-  if (a->n_lscols) {  // first rows of the labelset-derived values, from the per-labelset memo of k_header
-    LsFirstArgs lf{};
-    lf.first_ls = P.first_ls; lf.n_labelsets = P.n_labelsets; lf.lsmat = a->d_lsmat.as<uint32_t>();
-    lf.n_lscols = std::max<uint32_t>(1, a->n_lscols); lf.n_ls = a->n_lscols;
-    for (uint32_t c = 0; c < a->n_lscols; c++) lf.col_first[c] = P.col_first[c];
-    launch_chain(a, k_ls_first, dim3((unsigned)(small_grid(a, (uint64_t)lf.n_labelsets * lf.n_ls))), s, lf);
+  if (P.n_names) {  // check the column plan and apply it: key matrix and first rows of the labelset-derived values
+    LsPlanArgs lp{};
+    lp.first_ls = P.first_ls; lp.n_labelsets = P.n_labelsets;
+    lp.off = a->m_ls_off.ptr(); lp.pairs = (const uint2*)a->m_ls_pairs.ptr();
+    lp.n_cols = a->n_lscols; lp.rank = P.ls_rank; lp.keys = P.ls_keys; lp.n_used = P.ls_used; lp.used_names = P.used_names;
+    lp.ctr = a->d_ctr.as<Counters>();
+    for (uint32_t c = 0; c < a->n_lscols; c++) { lp.plan_ord[c] = a->cols[c].ord; lp.col_first[c] = P.col_first[c]; }
+    launch_chain(a, k_ls_plan, dim3((unsigned)(small_grid(a, P.n_labelsets))), s, lp);
     a->tm[T_LABELS].launches++;
   }
   if (P.v1) { k_kind_ranks<<<1, 32, 0, s>>>(a->v1_first_kind, a->d_kindtab.as<uint32_t>(), a->v1_kindrank, a->v1_kind_order, a->v1_n_kind_dict); a->tm[T_LABELS].launches++; }
@@ -1633,6 +1691,7 @@ static int pass_finish(pa_agg* a) {
   cudaStream_t s = a->s_comp;
   Counters* ctr = a->d_ctr.as<Counters>();
   CK(cudaMemcpyAsync(a->h_ctr_pinned, ctr, sizeof(Counters), cudaMemcpyDeviceToHost, s));
+  if (a->P.used_names) CK(cudaMemcpyAsync(a->h_used, a->P.used_names, (a->P.n_names + 31) / 32 * 4, cudaMemcpyDeviceToHost, s));
   CK(cudaEventRecord(a->tm[T_TOTAL].b, s));
   CK(cudaStreamSynchronize(s));
   CK(cudaGetLastError());
@@ -1685,6 +1744,7 @@ static int process_once(pa_agg* a) {
 
 static int check_batch_errors(pa_agg* a, uint32_t e) {
   if (e & ERR_TABLE_FULL) return a->fail(PA_ENOMEM, "stack table overflow");
+  if (e & ERR_LABEL_PLAN) return a->fail(PA_EIO, "label column plan: a used label name is still not planned after the redo");
   if (e & ERR_INDEX_OVERFLOW) return a->fail(PA_ERANGE, "location-index stream exceeds int32 (reporter/arrow_v2.go:233)");
   if (e & ERR_BAD_FRAME_ID) return a->fail(PA_EINVAL, "sample refers to an unregistered frame id");
   if (e & ERR_BAD_STRING_ID) return a->fail(PA_EINVAL, "sample refers to an unregistered string id");
@@ -1704,6 +1764,9 @@ static void remember_sizes(pa_agg* a) {  // adaptive table sizing for the next i
   for (uint32_t c = 0; c < a->n_label_cols; c++) if (a->cols[c].type == COL_TID) a->prev_tids = a->h_ctr.n_dict[c];
   a->retry_cap = 0;
   a->retry_tcap = 0;
+  a->used_prev = used_names(a);  // the next batch's label column prediction starts from these
+  a->names_planned = a->P.n_names;
+  a->plan_pending = false;
 }
 
 static int process(pa_agg* a) {
@@ -1711,15 +1774,19 @@ static int process(pa_agg* a) {
   CK(cudaSetDevice(a->device));
   a->merged_part = false;
   if (a->N == 0) { a->processed = true; a->last_unique = 0; memset(&a->h_ctr, 0, sizeof a->h_ctr); return PA_OK; }
-  int rc = upload_tables(a);
+  int rc = upload_tables(a, true);
   if (rc) return rc;
   for (int attempt = 0; attempt < 6; attempt++) {
     rc = process_once(a);
     if (rc) return rc;
-    if (!(a->h_ctr.err & ERR_TABLE_FULL)) break;
+    const uint32_t e = a->h_ctr.err;
+    if (!(e & (ERR_TABLE_FULL | ERR_LABEL_PLAN))) break;
     if (a->early.issued) CK(cudaStreamSynchronize(a->s_d2h));  // (k_header runs again and rewrites, with the same values, what is being copied out)
-    a->retry_cap = a->table_cap * 4;  // unique-stack / thread-id estimate was too small: grow and redo the batch
-    a->retry_tcap = a->tid_cap * 4;
+    if (e & ERR_TABLE_FULL) {
+      a->retry_cap = a->table_cap * 4;  // unique-stack / thread-id estimate was too small: grow and redo the batch
+      a->retry_tcap = a->tid_cap * 4;
+    }
+    if ((e & ERR_LABEL_PLAN) && (rc = replan_labels(a))) return rc;  // a used label name was not planned: plan the used ones, redo
   }
   if ((rc = check_batch_errors(a, a->h_ctr.err))) return rc;
   if (a->cfg.schema == PA_SCHEMA_V1) {
@@ -1932,7 +1999,8 @@ static int collect_nodes(pa_agg* a, const MergeView* mv, std::vector<Node>& cols
         out += n;
       }
     } else if (cp.type == COL_LS) {
-      for (uint32_t local : ord) v.push_back(cstr(cp.vals[local]));
+      const std::vector<uint32_t>& vals = a->ls.vals[cp.ord];
+      for (uint32_t local : ord) v.push_back(cstr(vals[local]));
     } else {
       for (uint32_t cid : ord) v.push_back(cstr(cid));
     }
@@ -2503,7 +2571,7 @@ static int stacktraces(pa_agg* a, const uint8_t* ids, uint64_t n, pa_agg_result*
   CK(cudaSetDevice(a->device));
   const double t0 = now_ms();
   a->hostbufs.clear();
-  int rc = upload_tables(a);  // frames may have been registered since the last flush
+  int rc = upload_tables(a, false);  // frames may have been registered since the last flush
   if (rc) return rc;
   cudaStream_t s = a->s_comp;
   const uint32_t n32 = (uint32_t)n;
@@ -2963,6 +3031,13 @@ int pa_agg_last_kernel_ms(const pa_agg* a, const char* name, double* ms, uint32_
       if (launches) *launches = a->tm[t].launches;
       return PA_OK;
     }
+  // the label column plan (ms is 0): labelset-derived columns planned for the last pass, and passes redone since creation
+  // because the prediction missed a name the batch's rows used
+  if (!strcmp(name, "label_columns") || !strcmp(name, "label_replans")) {
+    if (ms) *ms = 0;
+    if (launches) *launches = !strcmp(name, "label_columns") ? a->n_lscols : (uint32_t)std::min<uint64_t>(a->label_replans, 0xFFFFFFFFu);
+    return PA_OK;
+  }
   // PA_IPC_LZ4_FRAME_GPU merge groups (ms is 0): bytes of this member's parts that went to the owners of blocks crossing a part
   // border in the last pa_merge_plan
   if (!strcmp(name, "lz4_heads")) {

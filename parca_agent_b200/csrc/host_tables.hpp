@@ -173,9 +173,41 @@ struct FrameTableHost {
   }
 };
 
-// per-PID cached labels (the content of the `labels` LRU, parca_reporter.go:569) as canonical ids
+// per-PID cached labels (the content of the `labels` LRU, parca_reporter.go:569), append-only. Every distinct label name gets a
+// lifetime ordinal, every (name, value) pair a value id in that name's dictionary, and a labelset is its run of (ordinal, value
+// id) pairs in CSR form, which the device mirrors append-only. A batch's label column plan is a set of name ordinals.
 struct LabelSets {
-  std::vector<std::vector<std::pair<uint32_t, uint32_t>>> sets;  // (name cid, value cid)
+  std::vector<uint32_t> off{0};    // labelset -> its pairs [off[i], off[i + 1])
+  std::vector<uint32_t> pairs;     // two words per pair: name ordinal, value id
+  std::vector<uint32_t> name_cid;  // ordinal -> name canonical id
+  std::vector<std::vector<uint32_t>> vals;  // ordinal -> value id -> value canonical id
+  std::unordered_map<uint32_t, uint32_t> ord_of;              // name canonical id -> ordinal
+  std::vector<std::unordered_map<uint32_t, uint32_t>> val_of;  // ordinal -> value canonical id -> value id
+  uint32_t count() const { return (uint32_t)(off.size() - 1); }
+  uint32_t n_names() const { return (uint32_t)name_cid.size(); }
+
+  // one labelset of (name cid, value cid); a name that repeats keeps its last value
+  void add(const std::vector<std::pair<uint32_t, uint32_t>>& set) {
+    const size_t p0 = pairs.size();
+    for (auto& kv : set) {
+      auto it = ord_of.find(kv.first);
+      if (it == ord_of.end()) {
+        it = ord_of.emplace(kv.first, n_names()).first;
+        name_cid.push_back(kv.first);
+        vals.emplace_back();
+        val_of.emplace_back();
+      }
+      const uint32_t ord = it->second;
+      auto& vi = val_of[ord];
+      auto jt = vi.find(kv.second);
+      if (jt == vi.end()) { jt = vi.emplace(kv.second, (uint32_t)vals[ord].size()).first; vals[ord].push_back(kv.second); }
+      size_t p = p0;
+      while (p < pairs.size() && pairs[p] != ord) p += 2;
+      if (p == pairs.size()) { pairs.push_back(ord); pairs.push_back(jt->second); }
+      else pairs[p + 1] = jt->second;
+    }
+    off.push_back((uint32_t)(pairs.size() / 2));
+  }
 };
 
 }  // namespace pa

@@ -24,6 +24,7 @@ enum : uint32_t {
   ERR_SLICE_CAP = 256u,   // mode B: this shard's slice of the location-index stream exceeds its buffer
   ERR_MERGE_LOOKUP = 512u,  // mode B: a local stack is missing from the merged dictionary (internal error)
   ERR_BAD_STACK_ID = 1024u, // registered stacks: a row names a stack id that was not registered when the batch was processed
+  ERR_LABEL_PLAN = 2048u,   // a labelset the batch names carries a label name the column plan left out: the pass is redone
 };
 
 struct __align__(16) Key128 { unsigned long long hi, lo; };
@@ -266,7 +267,7 @@ struct HeaderArgs {
   // dictionary memo of the label columns: first row carrying each value. The first row of a value always
   // opens a run, so min over all rows == min over run starts; rows ascend with the grid here, which keeps the
   // atomics rare, and this DRAM-bound kernel has the issue slots to spare. nullptr = column disabled.
-  uint32_t* first_ls;            // per labelset id (expanded to the labelset-derived columns by k_ls_first)
+  uint32_t* first_ls;            // per labelset id (expanded to the labelset-derived columns by k_ls_plan)
   uint32_t* first_cpu;
   unsigned long long* tid_slots;
   uint32_t tid_mask;
@@ -1890,22 +1891,68 @@ __global__ void __launch_bounds__(kThreads) k_loc_chain(LocChainArgs a) {
   fo_map_dev(a.jobs[a.j_file]);
 }
 
-// labelset-derived label columns: first row of each value = min over the labelsets carrying it of the
-// labelset's first row (recorded by k_header). One thread per (labelset, column) matrix cell.
-struct LsFirstArgs {
+// The label column plan of the batch, checked and applied at the head of the label chain. For every labelset the batch names
+// (first_ls != kNull, recorded by k_header; in a merged batch all-reduced over the shards) a warp gives it a row of the key
+// matrix [used labelsets][planned columns], which KeyLs reaches through rank[], and walks its (name ordinal, value id) pairs:
+// each name sets its bit in the used-name bitmap; a planned one writes its value id into the row and lowers the first row of
+// its value (min over the labelsets carrying it of the labelset's first row); an unplanned one raises ERR_LABEL_PLAN, and the
+// host redoes the pass with exactly the used names planned. Rows are handed out by an atomic counter: the matrix is only an
+// indirection, so their order does not reach the output. Planned columns ascend by ordinal (binary search in shared memory).
+struct LsPlanArgs {
   const uint32_t* first_ls; uint32_t n_labelsets;
-  const uint32_t* lsmat; uint32_t n_lscols, n_ls;
-  uint32_t* col_first[kMaxCols];
+  const uint32_t* off; const uint2* pairs;  // the registered labelsets: pairs [off[ls], off[ls + 1]) of (name ordinal, value id)
+  uint32_t n_cols;                          // planned labelset-derived columns (the key matrix's row length)
+  uint32_t* rank;                           // [labelset] -> row of the key matrix (used labelsets only)
+  uint32_t* keys;                           // [row][n_cols] -> value id or kNull
+  uint32_t* n_used;                         // rows handed out (zeroed)
+  uint32_t* used_names;                     // bitmap over the name ordinals (zeroed)
+  Counters* ctr;
+  uint32_t plan_ord[kMaxCols];              // name ordinal of each planned column, ascending
+  uint32_t* col_first[kMaxCols];            // first-row table of each planned column, by value id
 };
-__global__ void __launch_bounds__(kThreads) k_ls_first(LsFirstArgs a) { pdl_enter();
-  uint32_t cells = a.n_labelsets * a.n_ls;
-  for (uint32_t i = blockIdx.x * kThreads + threadIdx.x; i < cells; i += gridDim.x * kThreads) {
-    uint32_t ls = i / a.n_ls, c = i % a.n_ls;
-    uint32_t f = a.first_ls[ls];
-    if (f == kNull) continue;  // labelset not used by this batch
-    uint32_t v = a.lsmat[(size_t)ls * a.n_lscols + c];
-    if (v != kNull && a.col_first[c][v] > f) atomicMin(&a.col_first[c][v], f);
+__global__ void __launch_bounds__(kThreads) k_ls_plan(LsPlanArgs a) { pdl_enter();
+  __shared__ uint32_t s_ord[kMaxCols];
+  for (uint32_t i = threadIdx.x; i < a.n_cols; i += kThreads) s_ord[i] = a.plan_ord[i];
+  __syncthreads();
+  const uint32_t lane = threadIdx.x & 31;
+  bool miss = false;
+  // 32 consecutive labelsets per warp and step: the trip count is uniform in the warp (the ballot needs all of it)
+  for (uint32_t base = blockIdx.x * kThreads + (threadIdx.x & ~31u); base < a.n_labelsets; base += gridDim.x * kThreads) {
+    const uint32_t ls = base + lane;
+    const uint32_t f = ls < a.n_labelsets ? a.first_ls[ls] : kNull;
+    const uint32_t used = __ballot_sync(0xFFFFFFFFu, f != kNull);
+    if (!used) continue;
+    uint32_t row0 = 0;
+    if (lane == 0) row0 = atomicAdd(a.n_used, (uint32_t)__popc(used));
+    row0 = __shfl_sync(0xFFFFFFFFu, row0, 0);
+    if (a.n_cols) {  // the warp's rows start all null (consecutive rows: coalesced stores)
+      uint32_t* rows = a.keys + (size_t)row0 * a.n_cols;
+      const uint32_t cells = (uint32_t)__popc(used) * a.n_cols;
+      for (uint32_t i = lane; i < cells; i += 32) rows[i] = kNull;
+    }
+    __syncwarp();
+    if (f != kNull) {
+      const uint32_t row = row0 + (uint32_t)__popc(used & ((1u << lane) - 1u));
+      a.rank[ls] = row;
+      uint32_t* keys = a.keys + (size_t)row * a.n_cols;
+      for (uint32_t p = a.off[ls], e = a.off[ls + 1]; p < e; p++) {
+        const uint2 kv = a.pairs[p];
+        uint32_t* w = &a.used_names[kv.x >> 5];
+        const uint32_t bit = 1u << (kv.x & 31);
+        if (!(*w & bit)) atomicOr(w, bit);
+        uint32_t lo = 0, hi = a.n_cols;
+        while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (s_ord[mid] < kv.x) lo = mid + 1; else hi = mid; }
+        if (lo < a.n_cols && s_ord[lo] == kv.x) {
+          keys[lo] = kv.y;
+          uint32_t* fp = a.col_first[lo] + kv.y;
+          if (*fp > f) atomicMin(fp, f);
+        } else {
+          miss = true;
+        }
+      }
+    }
   }
+  if (miss) atomicOr(&a.ctr->err, ERR_LABEL_PLAN);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1919,7 +1966,7 @@ struct ReeCol {
   uint32_t type, param;
   int* run_ends;       // Arrow: run_ends child
   uint32_t* run_keys;  // key of each run (kNull = null run)
-  uint32_t* first;     // dictionary first-ROW table (direct), filled by k_header / k_ls_first
+  uint32_t* first;     // dictionary first-ROW table (direct), filled by k_header / k_ls_plan
   unsigned long long* hslots;  // hashed variant (thread_id): (key << 32 | first row)
   uint32_t hmask;
   uint32_t nullable;
@@ -1933,7 +1980,8 @@ struct ReeArgs {
   uint32_t c_kind;               // first of the 8 kind columns
   const ReeCol* cols;
   const uint32_t* ls; const uint32_t* cpu; const uint32_t* tid; const uint32_t* comm; const uint8_t* kind;
-  const uint32_t* lsmat; uint32_t n_lscols;   // [labelset][LS column] -> value local id or kNull
+  const uint32_t* ls_rank;                    // [labelset] -> row of ls_keys (k_ls_plan)
+  const uint32_t* ls_keys; uint32_t n_lscols; // [row][LS column] -> value id or kNull
   const uint32_t* kindtab;                    // [8][8] -> class id or kNull
   uint32_t* partial;                          // [ncols][total warps]
   Counters* ctr;
@@ -2064,8 +2112,8 @@ __device__ __forceinline__ void ree_single(const ReeArgs& a, uint32_t c, bool ha
     if (nulls) atomicAdd(&a.ctr->n_null[c], nulls);
   }
 }
-struct KeyLs { const uint32_t* ls; const uint32_t* lsmat; uint32_t stride, c;
-  __device__ __forceinline__ void get(uint32_t r, uint32_t& k, bool& n) const { k = __ldg(&lsmat[(size_t)ls[r] * stride + c]); n = k == kNull; } };
+struct KeyLs { const uint32_t* ls; const uint32_t* rank; const uint32_t* keys; uint32_t stride, c;
+  __device__ __forceinline__ void get(uint32_t r, uint32_t& k, bool& n) const { k = __ldg(&keys[(size_t)__ldg(&rank[ls[r]]) * stride + c]); n = k == kNull; } };
 struct KeyU32 { const uint32_t* v;
   __device__ __forceinline__ void get(uint32_t r, uint32_t& k, bool& n) const { k = v[r]; n = false; } };
 struct KeyComm { const uint32_t* v;  // labels.Builder.Set(name, "") deletes the label: "" => null
@@ -2157,7 +2205,7 @@ __global__ void __launch_bounds__(kThreads) k_ree_col(ReeArgs a, ReeGroups group
     return;
   }
   switch (g.type) {
-    case COL_LS: ree_single<EMIT, MERGED, uint32_t>(a, g.col, true, KeyLs{a.ls, a.lsmat, a.n_lscols, g.param}); break;
+    case COL_LS: ree_single<EMIT, MERGED, uint32_t>(a, g.col, true, KeyLs{a.ls, a.ls_rank, a.ls_keys, a.n_lscols, g.param}); break;
     case COL_CPU: ree_single<EMIT, MERGED, uint32_t>(a, g.col, true, KeyU32{a.cpu}); break;
     case COL_TID: ree_single<EMIT, MERGED, uint32_t>(a, g.col, true, KeyU32{a.tid}); break;
     case COL_COMM: ree_single<EMIT, MERGED, uint32_t>(a, g.col, true, KeyComm{a.comm}); break;
@@ -2306,7 +2354,7 @@ __device__ __forceinline__ void ree_onepass(const ReeArgs& a, const ReeTiles& tl
 __global__ void __launch_bounds__(kThreads) k_ree_onepass(ReeArgs a, ReeGroups groups, ReeTiles tl) {
   const ReeGroup g = groups.g[blockIdx.y];
   switch (g.type) {
-    case COL_LS: ree_onepass<uint32_t>(a, tl, g.col, true, KeyLs{a.ls, a.lsmat, a.n_lscols, g.param}); break;
+    case COL_LS: ree_onepass<uint32_t>(a, tl, g.col, true, KeyLs{a.ls, a.ls_rank, a.ls_keys, a.n_lscols, g.param}); break;
     case COL_CPU: ree_onepass<uint32_t>(a, tl, g.col, true, KeyU32{a.cpu}); break;
     case COL_TID: ree_onepass<uint32_t>(a, tl, g.col, true, KeyU32{a.tid}); break;
     case COL_COMM: ree_onepass<uint32_t>(a, tl, g.col, true, KeyComm{a.comm}); break;

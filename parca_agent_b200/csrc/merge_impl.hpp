@@ -140,6 +140,7 @@ struct pa_merge {
   std::vector<MergeCol> cols_all;               // [world][ncols]
   std::vector<MergeCtl> mctl;                   // per local member
   uint32_t ncols = 0;
+  uint32_t retry_err = 0;                       // why merge_process_once asked for a redo: ERR_TABLE_FULL and / or ERR_LABEL_PLAN
   double ms_total = 0, ms_exchange_wait = 0;
   uint64_t nvlink_bytes = 0;                    // payload this process's members sent to other ranks during the last process()
   // ---- the stream last planned
@@ -622,7 +623,7 @@ static int merge_process_once(pa_merge* g, bool* retry) {
   auto cnt_of = [&](uint32_t from, uint32_t to) { return (uint64_t)hc[(size_t)from * cw + to]; };
   for (uint32_t r = 0; r < W; r++)
     if (hc[(size_t)r * cw + W + 1] & ERR_TABLE_FULL) { *retry = true; }
-  if (*retry) return PA_OK;  // some shard's local table was too small: every member redoes the batch with larger ones
+  if (*retry) { g->retry_err = ERR_TABLE_FULL; return PA_OK; }  // some shard's local table was too small: every member redoes the batch with larger ones
   if (g->group_retire) {  // a stale handle is seen only by the shard whose rows carry it: every rank stops here, before the exchange
     uint32_t e = 0;
     for (uint32_t r = 0; r < W; r++) e |= hc[(size_t)r * cw + W + 1];
@@ -822,7 +823,9 @@ static int merge_process_once(pa_merge* g, bool* retry) {
   if ((rc = t_allgather_host(g, csrc, 4, hb))) return rc;
   uint32_t err_any = 0;
   for (uint32_t r = 0; r < W; r++) err_any |= ((const uint32_t*)hb.data())[r];
-  if (err_any & ERR_TABLE_FULL) { *retry = true; return PA_OK; }
+  // (a label-plan miss is the same on every member: k_ls_plan ran on the all-reduced first_ls, so each member's used-name
+  // bitmap is the union of every shard's, and every member replans the same columns)
+  if (err_any & (ERR_TABLE_FULL | ERR_LABEL_PLAN)) { *retry = true; g->retry_err = err_any; return PA_OK; }
   for (size_t i = 0; i < L; i++) g->members[i]->h_ctr.err |= err_any;
   return PA_OK;
 }
@@ -1013,14 +1016,15 @@ static int merge_process(pa_merge* g) {
     MCK(cudaSetDevice(a->device));
     a->processed = false;
     a->merged_part = true;
-    if ((rc = upload_tables(a))) return g->fail(rc, a->err);
+    if ((rc = upload_tables(a, true))) return g->fail(rc, a->err);
   }
   StreamShare share(g);
   auto restore = [] {};
   // ---- rows of every shard -> global row ranges; registrations must be identical (ids are global)
   // (group stacks: n_stack_frames is the frames of the stacks not yet freed, since dead frames make arena lengths differ)
   struct Dims { uint64_t n, nf, store_entries, store_frames, n_stack_frames, stack_digest, stages;
-                uint32_t ncols, nlab, n_frames, n_cstr, n_labelsets, n_funcs, lz4, schema, group_stacks, n_stacks, group_retire; };
+                uint64_t plan_digest;  // the label column plan each member predicted (upload_tables)
+                uint32_t n_sample_cols, n_tail_cols, n_names, n_frames, n_cstr, n_labelsets, n_funcs, lz4, schema, group_stacks, n_stacks, group_retire; };
   std::vector<const void*> src(L);
   std::vector<uint8_t> hb;
   rc = PA_OK;
@@ -1028,7 +1032,8 @@ static int merge_process(pa_merge* g) {
     pa_agg* a = g->members[i];
     cudaSetDevice(a->device);
     Dims d{a->N, a->NF, a->store_entries, a->store_frames, a->P.stack_frames_live, a->P.stack_digest,
-           a->group_retire ? a->rs_stages : 0, (uint32_t)a->cols.size(), a->n_label_cols, a->P.n_frames, a->P.n_cstr, a->P.n_labelsets, a->P.n_funcs,
+           a->group_retire ? a->rs_stages : 0, a->plan_digest, a->n_label_cols - a->n_lscols, (uint32_t)a->cols.size() - a->n_label_cols, a->P.n_names,
+           a->P.n_frames, a->P.n_cstr, a->P.n_labelsets, a->P.n_funcs,
            g->lz4 ? 1u : 0u, (uint32_t)a->cfg.schema, a->group_stacks ? 1u : 0u, a->P.n_stacks, a->group_retire ? 1u : 0u};
     if (g->mb[i].gather_scratch.ensure(std::max<size_t>((size_t)(W + 1) * sizeof(Dims), 256)) != cudaSuccess) { rc = g->fail(PA_ENOMEM, "device allocation failed"); break; }
     // staged through the tail of the gather scratch (the head receives the gathered block)
@@ -1064,8 +1069,8 @@ static int merge_process(pa_merge* g) {
   g->NT = 0; g->NFT = 0;
   for (uint32_t r = 0; r < W; r++) {
     g->n_rows[r] = dims[r].n; g->nf[r] = dims[r].nf; g->row_base[r] = g->NT; g->NT += dims[r].n; g->NFT += dims[r].nf;
-    if (dims[r].ncols != dims[0].ncols || dims[r].nlab != dims[0].nlab || dims[r].n_frames != dims[0].n_frames || dims[r].n_cstr != dims[0].n_cstr ||
-        dims[r].n_labelsets != dims[0].n_labelsets || dims[r].n_funcs != dims[0].n_funcs) {
+    if (dims[r].n_sample_cols != dims[0].n_sample_cols || dims[r].n_tail_cols != dims[0].n_tail_cols || dims[r].n_names != dims[0].n_names ||
+        dims[r].n_frames != dims[0].n_frames || dims[r].n_cstr != dims[0].n_cstr || dims[r].n_labelsets != dims[0].n_labelsets || dims[r].n_funcs != dims[0].n_funcs) {
       restore();
       return g->fail(PA_EINVAL, "the shards of a merged batch must carry identical string / frame / labelset registrations");
     }
@@ -1074,11 +1079,18 @@ static int merge_process(pa_merge* g) {
   // group stacks: the rings hold no frames; the merged location-index stream, and each shard's slice of it, is bounded by the
   // frames of the (identical) registered stacks not yet freed, which every stack a row may name belongs to
   if (g->group_stacks) g->NFT = dims[0].n_stack_frames;
-  g->ncols = dims[0].ncols;
+  // The label column plan must be the same on every member: the edge / run exchanges pair columns by index. Members predict it
+  // from their own last batch, which differs when one of them flushed alone since the last merged batch; then all plan cold.
+  bool same_plan = true;
+  for (uint32_t r = 0; r < W; r++) same_plan &= dims[r].plan_digest == dims[0].plan_digest;
+  for (size_t i = 0; i < L && !same_plan; i++)
+    if ((rc = plan_cold(g->members[i]))) { restore(); return g->fail(rc, g->members[i]->err); }
+  g->ncols = (uint32_t)g->members[0]->cols.size();
   if (g->NT > 0x7FFFFFFFull) { restore(); return g->fail(PA_ERANGE, "merged batch exceeds the int32 row limit of run ends / ListView offsets"); }
-  if (g->NT == 0) {  // (like one aggregator's empty batch: no access to the store)
+  if (g->NT == 0) {  // (like one aggregator's empty batch: no access to the store, and the label column prediction stands)
     for (size_t i = 0; i < L; i++) {
       pa_agg* a = g->members[i];
+      a->plan_pending = false;
       a->processed = true; a->last_unique = 0; a->store_frames_sent = 0; a->store_refs_sent = 0;
       memset(&a->h_ctr, 0, sizeof(Counters));
     }
@@ -1091,11 +1103,18 @@ static int merge_process(pa_merge* g) {
   for (int attempt = 0; attempt < 6; attempt++) {
     rc = merge_process_once(g, &retry);
     if (rc || !retry) break;
-    for (size_t i = 0; i < L; i++) { g->members[i]->retry_cap = g->members[i]->table_cap * 4; g->members[i]->retry_tcap = g->members[i]->tid_cap * 4; }
+    for (size_t i = 0; i < L && !rc; i++) {
+      pa_agg* a = g->members[i];
+      if (g->retry_err & ERR_TABLE_FULL) { a->retry_cap = a->table_cap * 4; a->retry_tcap = a->tid_cap * 4; }
+      if ((g->retry_err & ERR_LABEL_PLAN) && (rc = replan_labels(a))) rc = g->fail(rc, a->err);
+    }
+    if (rc) break;
+    g->ncols = (uint32_t)g->members[0]->cols.size();
   }
   restore();
   if (rc) return rc;
-  if (retry) return g->fail(PA_ENOMEM, "stack / thread-id table overflow");
+  if (retry && (g->retry_err & ERR_TABLE_FULL)) return g->fail(PA_ENOMEM, "stack / thread-id table overflow");
+  if (retry) return g->fail(check_batch_errors(g->members[0], g->retry_err), g->members[0]->err);  // (the label plan still missed)
   for (size_t i = 0; i < L; i++) {
     pa_agg* a = g->members[i];
     if ((rc = check_batch_errors(a, a->h_ctr.err))) return g->fail(rc, a->err);
