@@ -130,9 +130,6 @@ struct Pass {
   std::vector<ReeCol> rc;
   ReeArgs ra{};
   ReeGroups rg{};        // every column group
-  ReeGroups rg_single{}; // the groups the one-sweep kernel encodes (everything but the kind-derived columns)
-  ReeGroups rg_kind{};   // the kind-derived group alone
-  ReeTiles tiles{};
 };
 
 struct pa_agg {
@@ -140,8 +137,6 @@ struct pa_agg {
   std::string err;
   int device = 0, sms = 148, G = 592;
   cudaStream_t s_copy = nullptr, s_comp = nullptr, s_aux = nullptr, s_d2h = nullptr;
-  cudaStream_t s_copy2 = nullptr;  // PA_COPY_STREAMS=2 (experiment): odd chunks of the id upload go through a second copy stream
-  cudaEvent_t ev_copy2 = nullptr;
   cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
   // Early copy-out during a flush (XXH64 mode, v2, more than one chunk): all headers are uploaded first, k_header and the label
   // chain run while the frame ids are still uploading, and stacktrace_id / value / timestamp leave for the host on s_d2h as soon
@@ -155,16 +150,11 @@ struct pa_agg {
     uint64_t dist_stoff = 0, dist_stsize = 0, dist_stream = 0;  // second wave (collect): list offsets / sizes and the location-index stream sit right before stacktrace_id
   } early;
   bool early_enabled = true, early_force = false;
-  bool use_pdl = false;  // PA_PDL=1: the small dependent kernels of the rank / location / label chains are launched with programmatic stream serialization
   cudaEvent_t ev_hdr_all = nullptr, ev_hdr_done = nullptr, ev_early = nullptr, ev_early_done = nullptr;
   std::vector<cudaEvent_t> hash_ev;
   uint8_t* h_early = nullptr;  // pinned: Counters, then the run keys of the eight kind-derived columns
   static constexpr uint32_t kEarlyMaxRuns = 512;
-  bool use_onepass = false;  // PA_REE_ONEPASS=1: label columns run-end encoded in one sweep with decoupled look-back (measured SLOWER than count + emit: 1.18 vs 0.39 ms on config 2, DESIGN section 7)
-  bool use_chain = false;    // PA_CHAIN=1: the stack-rank / dictionary chains as two persistent kernels with grid barriers instead of ~30 launches (measured no faster: DESIGN section 7)
-  int ree_blocks = 8;        // blocks per SM of the two run-end passes (PA_REE_BLOCKS_PER_SM)
-  bool fork_early = false;   // PA_FORK_EARLY=1: the label chain starts right after the header pass and runs beside the hash kernel
-  bool forked_early = false;
+  bool forked_early = false;  // headers-first staging: the label chain was forked right after the header pass, beside the hash kernel
   bool serial = false;       // PA_SERIAL=1: the label chain stays on the compute stream (per-group timings do not overlap)
   Pass P;
   bool merged_part = false;  // the processed batch is one shard of a merged record (collected through pa_merge_collect)
@@ -311,10 +301,6 @@ static void fatal_backtrace(int sig) {
   signal(sig, SIG_DFL);
   raise(sig);
 }
-// The one-sweep run-end kernel is persistent (tiles by ticket) and would fill the register file with 4 blocks per SM; asking
-// for 72 KB of (unused) dynamic shared memory holds it at 3, which leaves room for the two blocks per SM of the rank /
-// dictionary chain kernels that run beside it on the high-priority stream.
-static constexpr int kOnepassPadSmem = 72 * 1024;
 static uint64_t pow2_at_least(uint64_t v) { uint64_t p = 1; while (p < v) p <<= 1; return p; }
 
 #define CK(expr)                                                        \
@@ -488,7 +474,6 @@ int pa_agg_create(const pa_agg_config* cfg, pa_agg** out) {
     for (auto& v : kVariants) if (strcmp(hv, v.name) == 0) a->hash_variant = v.id;
   }
   if (cudaFuncSetAttribute(k_hash_insert_staged, cudaFuncAttributeMaxDynamicSharedMemorySize, kHashStagedSmem) != cudaSuccess) return bail(PA_EIO);
-  if (cudaFuncSetAttribute(k_ree_onepass, cudaFuncAttributeMaxDynamicSharedMemorySize, kOnepassPadSmem) != cudaSuccess) return bail(PA_EIO);
   if (cudaFuncSetAttribute(k_hash_insert_bulk<4, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BulkSmem<4, 3>)) != cudaSuccess) return bail(PA_EIO);
   if (cudaFuncSetAttribute(k_hash_insert_tma<16, 3, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TmaSmem<16, 3, 8>)) != cudaSuccess) return bail(PA_EIO);
   if (cudaFuncSetAttribute(k_hash_insert_tma<12, 4, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TmaSmem<12, 4, 8>)) != cudaSuccess) return bail(PA_EIO);
@@ -501,9 +486,6 @@ int pa_agg_create(const pa_agg_config* cfg, pa_agg** out) {
   if (cudaFuncSetAttribute(k_hash_insert_tmag<6, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TmagSmem<6, 4>)) != cudaSuccess) return bail(PA_EIO);
   if (cudaFuncSetAttribute(k_hash_insert_bulk<6, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(BulkSmem<6, 2>)) != cudaSuccess) return bail(PA_EIO);
   if (cudaStreamCreateWithFlags(&a->s_copy, cudaStreamNonBlocking) != cudaSuccess) return bail(PA_EIO);
-  if (const char* cs = getenv("PA_COPY_STREAMS")) {
-    if (atoi(cs) >= 2 && (cudaStreamCreateWithFlags(&a->s_copy2, cudaStreamNonBlocking) != cudaSuccess || cudaEventCreateWithFlags(&a->ev_copy2, cudaEventDisableTiming) != cudaSuccess)) return bail(PA_EIO);
-  }
   int prio_lo = 0, prio_hi = 0;
   cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi);  // numerically lower = higher priority
   // the compute stream carries the chain of short dependent launches (stack rank, dictionaries): its blocks are scheduled
@@ -516,16 +498,11 @@ int pa_agg_create(const pa_agg_config* cfg, pa_agg** out) {
   cudaEventCreateWithFlags(&a->ev_early, cudaEventDisableTiming);
   cudaEventCreateWithFlags(&a->ev_early_done, cudaEventDisableTiming);
   if (cudaHostAlloc((void**)&a->h_early, sizeof(Counters) + 8 * pa_agg::kEarlyMaxRuns * 4, cudaHostAllocDefault) != cudaSuccess) return bail(PA_ENOMEM);
-  if (const char* e = getenv("PA_PDL")) a->use_pdl = atoi(e) != 0;
   if (getenv("PA_NO_EARLY_D2H")) a->early_enabled = false;
   if (getenv("PA_EARLY_D2H_ALWAYS")) a->early_force = true;  // tests: take the early path even when the (tiny) upload is already over
   cudaEventCreateWithFlags(&a->ev_fork, cudaEventDisableTiming);
   cudaEventCreateWithFlags(&a->ev_join, cudaEventDisableTiming);
   if (const char* sv = getenv("PA_SERIAL")) a->serial = sv[0] == '1';
-  if (const char* sv = getenv("PA_FORK_EARLY")) a->fork_early = sv[0] == '1';
-  if (const char* sv = getenv("PA_CHAIN")) a->use_chain = sv[0] == '1';
-  if (const char* sv = getenv("PA_REE_ONEPASS")) a->use_onepass = sv[0] == '1';
-  if (const char* sv = getenv("PA_REE_BLOCKS_PER_SM")) a->ree_blocks = std::max(1, std::min(8, atoi(sv)));
   cudaEventCreate(&a->ev_h2d0);
   cudaEventCreate(&a->ev_h2d1);
   cudaEventCreate(&a->ev_d2h0);
@@ -618,8 +595,6 @@ void pa_agg_destroy(pa_agg* a) {
   if (a->rs_tm.b) cudaEventDestroy(a->rs_tm.b);
   if (a->ev_fork) cudaEventDestroy(a->ev_fork);
   if (a->ev_join) cudaEventDestroy(a->ev_join);
-  if (a->s_copy2) { cudaStreamSynchronize(a->s_copy2); cudaStreamDestroy(a->s_copy2); }
-  if (a->ev_copy2) cudaEventDestroy(a->ev_copy2);
   if (a->s_copy) cudaStreamDestroy(a->s_copy);
   if (a->s_comp) cudaStreamDestroy(a->s_comp);
   if (a->s_aux) cudaStreamDestroy(a->s_aux);
@@ -881,14 +856,12 @@ static int stage_async(pa_agg* a) {
     // reads those few stacks from the mapped pinned ring over PCIe (U*F*8 bytes instead of N*F*8).
     // Registered stacks: the ring holds headers only; the frames are in the device arena already.
     if (fend > fdone && upload_ids)
-      CK(cudaMemcpyAsync(a->d_frames.as<uint8_t>() + fdone * a->idb, (const uint8_t*)r.frames + fdone * a->idb, (fend - fdone) * a->idb, cudaMemcpyHostToDevice,
-                         (a->s_copy2 && a->early.hdr_first && (k & 1)) ? a->s_copy2 : a->s_copy));
+      CK(cudaMemcpyAsync(a->d_frames.as<uint8_t>() + fdone * a->idb, (const uint8_t*)r.frames + fdone * a->idb, (fend - fdone) * a->idb, cudaMemcpyHostToDevice, a->s_copy));
     fdone = fend;
-    CK(cudaEventRecord(a->chunk_ev[k], (a->s_copy2 && a->early.hdr_first && (k & 1)) ? a->s_copy2 : a->s_copy));
+    CK(cudaEventRecord(a->chunk_ev[k], a->s_copy));
     a->chunk_rows.emplace_back(r0, r1);
     a->chunk_frames_end.push_back(fend);
   }
-  if (a->s_copy2) { CK(cudaEventRecord(a->ev_copy2, a->s_copy2)); CK(cudaStreamWaitEvent(a->s_copy, a->ev_copy2, 0)); }  // s_copy stands for both from here on
   CK(cudaEventRecord(a->ev_h2d1, a->s_copy));
   return PA_OK;
 }
@@ -904,25 +877,13 @@ static void release_staged(pa_agg* a) {
   }
 }
 
-// launch of a chain kernel (every one of them starts with pdl_enter())
-template <class... KArgs, class... Args>
-static void launch_chain(const pa_agg* a, void (*k)(KArgs...), dim3 grid, cudaStream_t s, Args... args) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = grid; cfg.blockDim = dim3(kThreads); cfg.dynamicSmemBytes = 0; cfg.stream = s;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  at[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = at; cfg.numAttrs = a->use_pdl ? 1 : 0;
-  cudaLaunchKernelEx(&cfg, k, KArgs(args)...);
-}
-
 template <class F>
 static void launch_scan(pa_agg* a, F f, int njobs, Timer& t, int gx, cudaStream_t s, DBuf& scratch) {
   if (gx <= 0) gx = a->G;
   dim3 grid(gx, njobs);
   typename F::T* partial = scratch.as<typename F::T>();  // per-block totals: two concurrent scans need two scratch buffers
-  launch_chain(a, k_scan_reduce<F>, grid, s, f, partial);
-  launch_chain(a, k_scan_emit<F>, grid, s, f, partial);
+  k_scan_reduce<F><<<grid, kThreads, 0, s>>>(f, partial);
+  k_scan_emit<F><<<grid, kThreads, 0, s>>>(f, partial);
   t.launches += 2;
 }
 // grid for a pass over at most `bound` elements: >= 2048 elements per CTA, never more than the full grid
@@ -1076,12 +1037,12 @@ static int upload_tables(pa_agg* a, bool plan_batch) {
 static void run_fo_jobs(pa_agg* a, const FoJob* djobs, int first, int count, bool need_min, Timer& t, uint64_t elem_bound, uint64_t table_bound,
                         bool do_map, cudaStream_t s, DBuf& scratch) {
   const int ge = small_grid(a, elem_bound), gt = small_grid(a, table_bound), gw = small_grid(a, elem_bound / 32 + 1);
-  launch_chain(a, k_fo_zero, dim3(gw, count), s, djobs + first);
-  if (need_min) { launch_chain(a, k_fo_min, dim3(ge, count), s, djobs + first); t.launches++; }
-  launch_chain(a, k_fo_bits, dim3(gt, count), s, djobs + first);
+  k_fo_zero<<<dim3(gw, count), kThreads, 0, s>>>(djobs + first);
+  if (need_min) { k_fo_min<<<dim3(ge, count), kThreads, 0, s>>>(djobs + first); t.launches++; }
+  k_fo_bits<<<dim3(gt, count), kThreads, 0, s>>>(djobs + first);
   launch_scan(a, FoWordsF{djobs + first, -1}, count, t, gw, s, scratch);
-  launch_chain(a, k_fo_assign, dim3(gt, count), s, djobs + first);
-  if (do_map) { launch_chain(a, k_fo_map, dim3(ge, count), s, djobs + first); t.launches++; }
+  k_fo_assign<<<dim3(gt, count), kThreads, 0, s>>>(djobs + first);
+  if (do_map) { k_fo_map<<<dim3(ge, count), kThreads, 0, s>>>(djobs + first); t.launches++; }
   t.launches += 3;
 }
 
@@ -1336,9 +1297,6 @@ static int pass_plan(pa_agg* a, const MergeDims* md) {
   want(&a->lo.address, Pn * 8); want(&a->lo.line_off, Pn * 4); want(&a->lo.line_size, Pn * 4); want(&a->lo.line_valid, (Pn / 32 + 2) * 4);
   want(&a->lo.line_no, Pn * 8);
   if (md) want(&P.edge_keys, (size_t)ncols * 32, 1);
-  P.tiles = ReeTiles{};
-  P.tiles.n_tiles = (uint32_t)((N + kTileRows - 1) / kTileRows);
-  if (!md) { want(&P.tiles.desc, (size_t)ncols * std::max<uint32_t>(P.tiles.n_tiles, 1) * 8, 1); want(&P.tiles.next, (size_t)ncols * 4, 1); }
   P.col_first.assign(ncols, nullptr); P.col_rank.assign(ncols, nullptr); P.col_bits.assign(ncols, nullptr); P.col_wp.assign(ncols, nullptr);
   a->tid_slots = nullptr; a->tid_rank = nullptr;
   for (uint32_t c = 0; c < ncols; c++) {
@@ -1440,12 +1398,6 @@ static int pass_plan(pa_agg* a, const MergeDims* md) {
     if (cp.type == COL_KIND && cp.param != 0) continue;
     rg.g[rg.n++] = ReeGroup{cp.type, c, cp.param};
   }
-  P.rg_single = ReeGroups{};
-  P.rg_kind = ReeGroups{};
-  for (uint32_t i = 0; i < rg.n; i++) {
-    if (rg.g[i].type == COL_KIND) P.rg_kind.g[P.rg_kind.n++] = rg.g[i];
-    else P.rg_single.g[P.rg_single.n++] = rg.g[i];
-  }
   int rcu = upload_descriptors(a, jobs.data(), jobs.size() * sizeof(FoJob), rc.data(), rc.size() * sizeof(ReeCol));
   if (rcu) return rcu;
   ra.cols = a->d_cols.as<ReeCol>();
@@ -1527,7 +1479,6 @@ static int pass_front(pa_agg* a) {
   if (resident) {
     if (N) launch_header(0, N, a->NF);  // whole resident batch: one launch per pass
     CK(cudaEventRecord(a->tm[T_HEADER].b, s));
-    if (a->fork_early && !a->serial && !P.v1 && !P.merged) { CK(cudaEventRecord(a->ev_fork, s)); a->forked_early = true; }
     CK(cudaEventRecord(a->tm[T_HASH].a, s));
     if (!provided && N) launch_hash(0, N);
     CK(cudaEventRecord(a->tm[T_HASH].b, s));
@@ -1563,32 +1514,19 @@ static int pass_rank_single(pa_agg* a) {
   StackSlot* tab = a->d_table.as<StackSlot>();
   const int G = a->G;
   CK(cudaEventRecord(a->tm[T_RANK].a, s));
-  if (a->use_chain && !P.v1) {  // one persistent kernel: 5 grid barriers instead of 7 dependent launches
-    RankChainArgs ra{};
-    ra.tab = tab; ra.claimed = P.claimed; ra.ctr = ctr; ra.rowbits = P.rowbits; ra.row_wprefix = P.row_wprefix; ra.n_words = (uint32_t)((N + 31) / 32);
-    ra.nframes = a->d_nfr.as<uint16_t>(); ra.uniq_row = a->d_uniq_row.as<uint32_t>(); ra.uniq_slot = P.uniq_slot; ra.uniq_size = P.uniq_size;
-    ra.partial32 = a->d_partial.as<uint32_t>(); ra.partial64 = (unsigned long long*)(a->d_partial.as<uint8_t>() + 65536);
-    ra.n_rows = (uint32_t)N; ra.slot_of_row = a->d_slot.as<uint32_t>(); ra.st_offsets = a->d_stoff.as<int>(); ra.st_sizes = a->d_stsize.as<int>();
-    ra.frames = a->src_frames; ra.frame_off = a->d_foff.as<unsigned long long>(); ra.n_frames_registered = P.n_frames;
-    ra.ustream = a->d_ustream.as<uint32_t>(); ra.loc_first = a->loc_first; ra.narrow = a->idb == 4 ? 1u : 0u;
-    k_rank_chain<<<a->sms * 2, kThreads, 0, s>>>(ra);
-    a->tm[T_RANK].launches += 1;
-    CK(cudaEventRecord(a->tm[T_RANK].b, s));
-    return PA_OK;
-  }
   const int Gw = small_grid(a, N / 32 + 1), Gu = small_grid(a, std::min<uint64_t>(N, P.cap / 2));
-  launch_chain(a, k_stack_bits, dim3((unsigned)(Gu)), s, tab, P.claimed, &ctr->n_claimed, P.rowbits);
+  k_stack_bits<<<Gu, kThreads, 0, s>>>(tab, P.claimed, &ctr->n_claimed, P.rowbits);
   launch_scan(a, WordsF{P.rowbits, P.row_wprefix, (uint32_t)((N + 31) / 32), &ctr->n_unique}, 1, a->tm[T_RANK], Gw, s, a->d_partial);
-  launch_chain(a, k_stack_assign, dim3((unsigned)(Gu)), s, tab, P.claimed, &ctr->n_claimed, P.rowbits, P.row_wprefix, a->d_nfr.as<uint16_t>(), a->d_uniq_row.as<uint32_t>(), P.uniq_slot, P.uniq_size);
+  k_stack_assign<<<Gu, kThreads, 0, s>>>(tab, P.claimed, &ctr->n_claimed, P.rowbits, P.row_wprefix, a->d_nfr.as<uint16_t>(), a->d_uniq_row.as<uint32_t>(), P.uniq_slot, P.uniq_size);
   launch_scan(a, UniqOffsetF{ctr, ctr, P.uniq_size, P.uniq_slot, tab}, 1, a->tm[T_RANK], Gu, s, a->d_partial);
   a->tm[T_RANK].launches += 2;
-  launch_chain(a, k_rows_materialize, dim3((unsigned)(G)), s, (uint32_t)N, a->d_slot.as<uint32_t>(), tab, a->d_stoff.as<int>(), a->d_stsize.as<int>(), P.v1 ? a->v1_ord : nullptr);
+  k_rows_materialize<<<G, kThreads, 0, s>>>((uint32_t)N, a->d_slot.as<uint32_t>(), tab, a->d_stoff.as<int>(), a->d_stsize.as<int>(), P.v1 ? a->v1_ord : nullptr);
   if (P.v1) {  // v1 has no inline stacktraces: only the dictionary of unique stack ids
     k_gather_ids<<<small_grid(a, std::min<uint64_t>(N, P.cap / 2) + 1), kThreads, 0, s>>>(ctr, a->d_uniq_row.as<uint32_t>(), a->d_uuid.as<uint8_t>(), a->v1_ids, a->v1_id_off);
     a->tm[T_RANK].launches++;
   } else {
-    launch_chain(a, k_gather_unique, dim3((unsigned)(G)), s, ctr, a->d_uniq_row.as<uint32_t>(), a->d_slot.as<uint32_t>(), tab, a->src_frames,
-                                           a->d_foff.as<unsigned long long>(), P.n_frames, a->d_ustream.as<uint32_t>(), a->loc_first, ctr, a->idb == 4 ? 1u : 0u);
+    k_gather_unique<<<G, kThreads, 0, s>>>(ctr, a->d_uniq_row.as<uint32_t>(), a->d_slot.as<uint32_t>(), tab, a->src_frames, a->d_foff.as<unsigned long long>(), P.n_frames,
+                                           a->d_ustream.as<uint32_t>(), a->loc_first, ctr, a->idb == 4 ? 1u : 0u);
   }
   a->tm[T_RANK].launches += 2;
   CK(cudaEventRecord(a->tm[T_RANK].b, s));
@@ -1605,20 +1543,12 @@ static int pass_locations(pa_agg* a) {
   const size_t Pn = P.Pn, S = P.S, FN = P.FN;
   CK(cudaEventRecord(a->tm[T_LOC].a, s));
   FrameTable ftd{(const unsigned long long*)a->m_addr.ptr(), a->m_type.ptr(), a->m_map.ptr(), a->m_bid.ptr(), (const unsigned long long*)a->m_line.ptr(), a->m_func.ptr()};
-  if (!P.v1 && a->use_chain && !P.merged) {  // one persistent kernel: 21 grid barriers instead of 24 dependent launches
-    LocChainArgs la{};
-    la.jobs = djobs; la.j_loc = P.j_loc; la.j_type = P.j_type; la.j_file = P.j_file; la.ctr = ctr;
-    la.loc_order = a->loc_order; la.ft = ftd; la.lo = a->lo;
-    la.fn_order = a->fn_order; la.fn_file_cid = a->m_fnfile.ptr(); la.file_key = a->sd_keys[3];
-    la.partial = a->d_partial.as<uint32_t>();
-    k_loc_chain<<<a->sms * 2, kThreads, 0, s>>>(la);
-    a->tm[T_LOC].launches += 1;
-  } else if (!P.v1) {  // v1 carries no locations in the sample record
+  if (!P.v1) {  // v1 carries no locations in the sample record
     run_fo_jobs(a, djobs, P.j_loc, 1, false, a->tm[T_LOC], std::min<uint64_t>(P.NI, P.merged ? P.NI : P.cap * 32), Pn, true, s, a->d_partial);  // location index per unique-stack frame (in place over the gathered stream)
     launch_scan(a, LocLinesF{ctr, ctr, a->loc_order, ftd, a->lo}, 1, a->tm[T_LOC], small_grid(a, Pn), s, a->d_partial);
-    launch_chain(a, k_line_validity, dim3((unsigned)(std::max(1, std::min(G, (int)(Pn / 256 + 1))))), s, ctr, a->lo.line_size, a->lo.line_valid);
+    k_line_validity<<<std::max(1, std::min(G, (int)(Pn / 256 + 1))), kThreads, 0, s>>>(ctr, a->lo.line_size, a->lo.line_valid);
     run_fo_jobs(a, djobs, P.j_type, 4, true, a->tm[T_LOC], Pn, std::max(S, FN), true, s, a->d_partial);  // frame_type, mapping_file, mapping_build_id, function
-    launch_chain(a, k_func_keys, dim3((unsigned)(std::max(1, std::min(G, (int)(FN / 256 + 1))))), s, ctr, a->fn_order, a->m_fnfile.ptr(), a->sd_keys[3]);
+    k_func_keys<<<std::max(1, std::min(G, (int)(FN / 256 + 1))), kThreads, 0, s>>>(ctr, a->fn_order, a->m_fnfile.ptr(), a->sd_keys[3]);
     run_fo_jobs(a, djobs, P.j_file, 1, true, a->tm[T_LOC], FN, S, true, s, a->d_partial);  // function.filename
     a->tm[T_LOC].launches += 2;
   }
@@ -1639,34 +1569,16 @@ static int pass_labels_count(pa_agg* a, cudaStream_t s) {
     lp.n_cols = a->n_lscols; lp.rank = P.ls_rank; lp.keys = P.ls_keys; lp.n_used = P.ls_used; lp.used_names = P.used_names;
     lp.ctr = a->d_ctr.as<Counters>();
     for (uint32_t c = 0; c < a->n_lscols; c++) { lp.plan_ord[c] = a->cols[c].ord; lp.col_first[c] = P.col_first[c]; }
-    launch_chain(a, k_ls_plan, dim3((unsigned)(small_grid(a, P.n_labelsets))), s, lp);
+    k_ls_plan<<<small_grid(a, P.n_labelsets), kThreads, 0, s>>>(lp);
     a->tm[T_LABELS].launches++;
   }
   if (P.v1) { k_kind_ranks<<<1, 32, 0, s>>>(a->v1_first_kind, a->d_kindtab.as<uint32_t>(), a->v1_kindrank, a->v1_kind_order, a->v1_n_kind_dict); a->tm[T_LABELS].launches++; }
-  if (a->use_onepass && !P.merged) return PA_OK;  // single aggregator: dictionary ranks next, then one sweep (pass_labels_onepass)
-  const int Gr = a->sms * a->ree_blocks;  // latency-bound passes: fill every warp slot
+  const int Gr = a->sms * kReeBlocksPerSm;
   const dim3 ree_grid(Gr, P.rg.n);
-  if (P.merged) launch_chain(a, k_ree_col<false, true>, ree_grid, s, P.ra, P.rg);  // run counts (+ this shard's border keys)
-  else launch_chain(a, k_ree_col<false, false>, ree_grid, s, P.ra, P.rg);
-  launch_chain(a, k_ree_scan_partials, dim3((unsigned)(P.ncols)), s, P.ra, Gr * kWarps, 0u);
+  if (P.merged) k_ree_col<false, true><<<ree_grid, kThreads, 0, s>>>(P.ra, P.rg);  // run counts (+ this shard's border keys)
+  else k_ree_col<false, false><<<ree_grid, kThreads, 0, s>>>(P.ra, P.rg);
+  k_ree_scan_partials<<<P.ncols, kThreads, 0, s>>>(P.ra, Gr * kWarps, 0u);
   a->tm[T_LABELS].launches += 2;
-  return PA_OK;
-}
-// single aggregator: every label column (and the v1 stacktrace_id / timestamp columns) in ONE sweep with decoupled look-back;
-// the kind-derived group (one shared key, almost always a single run) keeps its count / scan / emit form
-static int pass_labels_onepass(pa_agg* a, cudaStream_t s) {
-  Pass& P = a->P;
-  const int Gr = a->sms * 8;
-  // tiles are handed out by ticket, so the grid only has to fill the machine once (56 registers: 4 blocks per SM)
-  if (P.rg_single.n) { k_ree_onepass<<<dim3((unsigned)std::max(1, std::min(Gr / 2, (int)(P.tiles.n_tiles / kWarps + 1))), P.rg_single.n), kThreads, a->serial ? 0 : kOnepassPadSmem, s>>>(P.ra, P.rg_single, P.tiles); a->tm[T_LABELS].launches++; }
-  if (P.rg_kind.n) {
-    const dim3 kg(a->sms * 4, 1);
-    launch_chain(a, k_ree_col<false, false>, kg, s, P.ra, P.rg_kind);
-    launch_chain(a, k_ree_scan_partials, dim3((unsigned)(8)), s, P.ra, (int)kg.x * kWarps, P.nlab);
-    launch_chain(a, k_ree_col<true, false>, kg, s, P.ra, P.rg_kind);
-    a->tm[T_LABELS].launches += 3;
-  }
-  CK(cudaEventRecord(a->tm[T_LABELS].b, s));
   return PA_OK;
 }
 static int pass_label_dicts(pa_agg* a, cudaStream_t s, DBuf& partial) {
@@ -1678,9 +1590,9 @@ static int pass_label_dicts(pa_agg* a, cudaStream_t s, DBuf& partial) {
 }
 static int pass_labels_emit(pa_agg* a, cudaStream_t s) {
   Pass& P = a->P;
-  const dim3 ree_grid(a->sms * a->ree_blocks, P.rg.n);
-  if (P.merged) launch_chain(a, k_ree_col<true, true>, ree_grid, s, P.ra, P.rg);   // run ends + final dictionary indices + validity bits
-  else launch_chain(a, k_ree_col<true, false>, ree_grid, s, P.ra, P.rg);
+  const dim3 ree_grid(a->sms * kReeBlocksPerSm, P.rg.n);
+  if (P.merged) k_ree_col<true, true><<<ree_grid, kThreads, 0, s>>>(P.ra, P.rg);   // run ends + final dictionary indices + validity bits
+  else k_ree_col<true, false><<<ree_grid, kThreads, 0, s>>>(P.ra, P.rg);
   a->tm[T_LABELS].launches += 1;
   CK(cudaEventRecord(a->tm[T_LABELS].b, s));
   return PA_OK;
@@ -1729,7 +1641,7 @@ static int process_once(pa_agg* a) {
   if ((rc = pass_locations(a))) return rc;
   if ((rc = pass_labels_count(a, s2))) return rc;
   if ((rc = pass_label_dicts(a, s2, fork ? a->d_partial2 : a->d_partial))) return rc;
-  if ((rc = a->use_onepass ? pass_labels_onepass(a, s2) : pass_labels_emit(a, s2))) return rc;
+  if ((rc = pass_labels_emit(a, s2))) return rc;
   // (the early copy-out is not worth starting when the upload has already finished: nothing left to hide behind)
   const bool early = fork && a->forked_early && a->early.hdr_first && !a->early.issued && !a->P.merged && a->out && !a->chunk_rows.empty() &&
                      (a->early_force || cudaEventQuery(a->chunk_ev[a->chunk_rows.size() - 1]) != cudaSuccess);

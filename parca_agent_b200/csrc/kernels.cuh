@@ -63,18 +63,10 @@ struct Counters {
   uint32_t n_dict[kMaxCols];
   uint32_t n_null[kMaxCols];
   uint32_t last_nonnull_plus1[kMaxCols];
-  uint32_t chain_bar[2];    // arrival counters of the two persistent chain kernels (k_rank_chain, k_loc_chain)
 };
 
 // ---------------------------------------------------------------------------------------------
 // small helpers
-// Programmatic dependent launch (PA_PDL=1): a chain kernel lets its successor in the stream be scheduled at once and then waits
-// until its own predecessor has completed and flushed — the launch latency of kernel i+1 overlaps the execution of kernel i.
-// Without the launch attribute both instructions are no-ops.
-__device__ __forceinline__ void pdl_enter() {
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-  asm volatile("griddepcontrol.wait;" ::: "memory");
-}
 // two funnel shifts (SHF) for any constant rotation; the generic (x << r) | (x >> (64 - r)) form compiled to four
 // instructions for r = 31 (shift, shift-as-IMAD, shift, LOP3), which is the rotation of every XXH64 round
 __device__ __forceinline__ unsigned long long rotl64(unsigned long long x, int r) {
@@ -1400,8 +1392,9 @@ __device__ __forceinline__ T block_exclusive_scan(T v, T* total) {
 // blockIdx.y selects an independent job; two launches per scan (reduce, emit). (A cooperative single-launch variant with grid-wide barriers
 // between the phases was measured and was slower than these pipelined launches: DESIGN.md section 7.)
 template <class F>
-__device__ __forceinline__ void scan_reduce_dev(const F& f, typename F::T* partial_of_job) {
+__global__ void __launch_bounds__(kThreads) k_scan_reduce(F f, typename F::T* partial) {
   typedef typename F::T T;
+  T* partial_of_job = partial + (size_t)blockIdx.y * gridDim.x;
   uint32_t n = f.n(), begin, end;
   block_range(n, &begin, &end);
   T acc = zero_of(T());
@@ -1410,19 +1403,20 @@ __device__ __forceinline__ void scan_reduce_dev(const F& f, typename F::T* parti
   block_exclusive_scan(acc, &tot);
   if (threadIdx.x == 0) partial_of_job[blockIdx.x] = tot;
 }
-// Emit phase. `partial_of_job` holds the per-block TOTALS written by scan_reduce_dev; every block sums the
+// Emit phase. `partial` holds the per-block TOTALS written by k_scan_reduce; every block sums the
 // totals of its predecessors itself (at most a few hundred values), which removes the separate
 // "scan the partials" launch; the last block also publishes the grand total.
 template <class F>
-__device__ __forceinline__ void scan_emit_dev(const F& f, const typename F::T* partial_of_job, int job) {
+__global__ void __launch_bounds__(kThreads) k_scan_emit(F f, const typename F::T* partial) {
   typedef typename F::T T;
+  const T* partial_of_job = partial + (size_t)blockIdx.y * gridDim.x;
   uint32_t n = f.n(), begin, end;
   block_range(n, &begin, &end);
   T mine = zero_of(T());
   for (uint32_t b = threadIdx.x; b < blockIdx.x; b += kThreads) mine = mine + partial_of_job[b];
   T run;
   block_exclusive_scan(mine, &run);  // run = sum of all preceding blocks' totals
-  if (blockIdx.x == gridDim.x - 1 && threadIdx.x == 0) f.total(job, run + partial_of_job[blockIdx.x]);
+  if (blockIdx.x == gridDim.x - 1 && threadIdx.x == 0) f.total((int)blockIdx.y, run + partial_of_job[blockIdx.x]);
   for (uint32_t tile = begin; tile < end; tile += kThreads) {
     uint32_t i = tile + threadIdx.x;
     bool in = i < end;
@@ -1433,28 +1427,17 @@ __device__ __forceinline__ void scan_emit_dev(const F& f, const typename F::T* p
     run = run + tot;
   }
 }
-template <class F>
-__global__ void __launch_bounds__(kThreads) k_scan_reduce(F f, typename F::T* partial) { pdl_enter();
-  scan_reduce_dev(f, partial + (size_t)blockIdx.y * gridDim.x);
-}
-template <class F>
-__global__ void __launch_bounds__(kThreads) k_scan_emit(F f, const typename F::T* partial) { pdl_enter();
-  scan_emit_dev(f, partial + (size_t)blockIdx.y * gridDim.x, (int)blockIdx.y);
-}
 
 // ---------------------------------------------------------------------------------------------
 // (1) unique stacks in first-occurrence order. The table holds each stack's first row; ordinals
 // come from a bitmap over rows (one bit per first occurrence) + a popcount prefix over its words,
 // so only table-sized and N/32-sized passes are needed (no scan over all rows).
-__device__ __forceinline__ void stack_bits_dev(const StackSlot* tab, const uint32_t* claimed, const uint32_t* n_claimed, uint32_t* rowbits) {
+__global__ void __launch_bounds__(kThreads) k_stack_bits(const StackSlot* tab, const uint32_t* claimed, const uint32_t* n_claimed, uint32_t* rowbits) {
   const uint32_t n = *n_claimed;
   for (uint32_t i = blockIdx.x * kThreads + threadIdx.x; i < n; i += gridDim.x * kThreads) {
     uint32_t f = 0xFFFFFFFFu - tab[claimed[i]].first_inv;
     atomicOr(&rowbits[f >> 5], 1u << (f & 31));
   }
-}
-__global__ void __launch_bounds__(kThreads) k_stack_bits(const StackSlot* tab, const uint32_t* claimed, const uint32_t* n_claimed, uint32_t* rowbits) { pdl_enter();
-  stack_bits_dev(tab, claimed, n_claimed, rowbits);
 }
 struct WordsF {  // exclusive popcount prefix over bitmap words
   typedef uint32_t T;
@@ -1468,15 +1451,9 @@ struct WordsF {  // exclusive popcount prefix over bitmap words
   __device__ void total(int, uint32_t t) const { *total_out = t; }
 };
 // nframes == nullptr (mode B, merged table): the slot already carries the size of the stack's first occurrence
-__device__ __forceinline__ void stack_assign_dev(StackSlot* tab, const uint32_t* claimed, const uint32_t* n_claimed, const uint32_t* rowbits,
-                                                 const uint32_t* wprefix, const uint16_t* nframes, uint32_t* uniq_row, uint32_t* uniq_slot, uint32_t* uniq_size);
 __global__ void __launch_bounds__(kThreads) k_stack_assign(StackSlot* tab, const uint32_t* claimed, const uint32_t* n_claimed, const uint32_t* rowbits,
                                                            const uint32_t* wprefix, const uint16_t* nframes, uint32_t* uniq_row, uint32_t* uniq_slot,
-                                                           uint32_t* uniq_size) { pdl_enter();
-  stack_assign_dev(tab, claimed, n_claimed, rowbits, wprefix, nframes, uniq_row, uniq_slot, uniq_size);
-}
-__device__ __forceinline__ void stack_assign_dev(StackSlot* tab, const uint32_t* claimed, const uint32_t* n_claimed, const uint32_t* rowbits,
-                                                 const uint32_t* wprefix, const uint16_t* nframes, uint32_t* uniq_row, uint32_t* uniq_slot, uint32_t* uniq_size) {
+                                                           uint32_t* uniq_size) {
   const uint32_t n = *n_claimed;
   for (uint32_t i = blockIdx.x * kThreads + threadIdx.x; i < n; i += gridDim.x * kThreads) {
     uint32_t sidx = claimed[i];
@@ -1511,12 +1488,8 @@ struct UniqOffsetF {  // startOffset := indices.Len() at each first occurrence (
 // (2) per-row ListView offset/size: hit => reuse the first occurrence's (offset,size) (arrow_v2.go:293-299)
 // v2: the ListView (offset, size) of each row; v1 (ord_out != nullptr): the row's stack ordinal, which is
 // both the run key and the dictionary index of the stacktrace_id column.
-__device__ __forceinline__ void rows_materialize_dev(uint32_t n_rows, const uint32_t* slot_of_row, const StackSlot* tab, int* st_offsets, int* st_sizes, uint32_t* ord_out);
 __global__ void __launch_bounds__(kThreads) k_rows_materialize(uint32_t n_rows, const uint32_t* slot_of_row, const StackSlot* tab,
-                                                               int* st_offsets, int* st_sizes, uint32_t* ord_out) { pdl_enter();
-  rows_materialize_dev(n_rows, slot_of_row, tab, st_offsets, st_sizes, ord_out);
-}
-__device__ __forceinline__ void rows_materialize_dev(uint32_t n_rows, const uint32_t* slot_of_row, const StackSlot* tab, int* st_offsets, int* st_sizes, uint32_t* ord_out) {
+                                                               int* st_offsets, int* st_sizes, uint32_t* ord_out) {
   const uint32_t stride = gridDim.x * kThreads * 4;
   for (uint32_t base = blockIdx.x * kThreads * 4; base < n_rows; base += stride) {
     uint32_t sl[4];
@@ -1595,18 +1568,10 @@ __global__ void __launch_bounds__(kThreads) k_count_stacks(uint32_t n_rows, cons
 __device__ __forceinline__ unsigned long long frame_at(const unsigned long long* frames, unsigned long long i, uint32_t narrow) {
   return narrow ? (unsigned long long)reinterpret_cast<const uint32_t*>(frames)[i] : frames[i];
 }
-__device__ __forceinline__ void gather_unique_dev(const Counters* ctr, const uint32_t* uniq_row, const uint32_t* slot_of_row, const StackSlot* tab,
-                                                  const unsigned long long* frames, const unsigned long long* frame_off, uint32_t n_frames_registered,
-                                                  uint32_t* ustream, uint32_t* loc_first, Counters* ctr_w, uint32_t narrow = 0);
 __global__ void __launch_bounds__(kThreads) k_gather_unique(const Counters* ctr, const uint32_t* uniq_row, const uint32_t* slot_of_row,
                                                             const StackSlot* tab, const unsigned long long* frames,
                                                             const unsigned long long* frame_off, uint32_t n_frames_registered,
-                                                            uint32_t* ustream, uint32_t* loc_first, Counters* ctr_w, uint32_t narrow) { pdl_enter();
-  gather_unique_dev(ctr, uniq_row, slot_of_row, tab, frames, frame_off, n_frames_registered, ustream, loc_first, ctr_w, narrow);
-}
-__device__ __forceinline__ void gather_unique_dev(const Counters* ctr, const uint32_t* uniq_row, const uint32_t* slot_of_row, const StackSlot* tab,
-                                                  const unsigned long long* frames, const unsigned long long* frame_off, uint32_t n_frames_registered,
-                                                  uint32_t* ustream, uint32_t* loc_first, Counters* ctr_w, uint32_t narrow) {
+                                                            uint32_t* ustream, uint32_t* loc_first, Counters* ctr_w, uint32_t narrow) {
   uint32_t nu = ctr->n_unique;
   int lane = threadIdx.x & 31;
   uint32_t warp = (blockIdx.x * kThreads + threadIdx.x) >> 5, nwarps = (gridDim.x * kThreads) >> 5;
@@ -1656,7 +1621,8 @@ struct FoJob {
 __device__ __forceinline__ uint32_t gtid() { return blockIdx.x * kThreads + threadIdx.x; }
 __device__ __forceinline__ uint32_t gstride() { return gridDim.x * kThreads; }
 
-__device__ __forceinline__ void fo_min_dev(const FoJob& j) {
+__global__ void __launch_bounds__(kThreads) k_fo_min(const FoJob* jobs) {
+  const FoJob& j = jobs[blockIdx.y];
   if (j.skip_min) return;
   uint32_t n = j.n_ptr ? *j.n_ptr : j.n_imm;
   for (uint32_t i = gtid(); i < n; i += gstride()) {
@@ -1665,11 +1631,13 @@ __device__ __forceinline__ void fo_min_dev(const FoJob& j) {
     if (j.first[key] > i) atomicMin(&j.first[key], i);  // hashed jobs (thread ids) record first rows in k_header
   }
 }
-__device__ __forceinline__ void fo_zero_dev(const FoJob& j) {  // clear only the bitmap words this batch will use
+__global__ void __launch_bounds__(kThreads) k_fo_zero(const FoJob* jobs) {  // clear only the bitmap words this batch will use
+  const FoJob& j = jobs[blockIdx.y];
   uint32_t nw = (j.n_ptr ? *j.n_ptr : j.n_imm) / 32 + 1;
   for (uint32_t i = gtid(); i < nw; i += gstride()) j.bitmap[i] = 0u;
 }
-__device__ __forceinline__ void fo_bits_dev(const FoJob& j) {
+__global__ void __launch_bounds__(kThreads) k_fo_bits(const FoJob* jobs) {
+  const FoJob& j = jobs[blockIdx.y];
   uint32_t entries = j.hashed ? j.hmask + 1 : j.universe;
   for (uint32_t e = gtid(); e < entries; e += gstride()) {
     uint32_t f;
@@ -1688,7 +1656,8 @@ struct FoWordsF {
   __device__ void emit(uint32_t i, uint32_t ex, uint32_t) const { J().wprefix[i] = ex; }
   __device__ void total(int job, uint32_t t) const { *jobs[sel >= 0 ? sel : job].n_unique = t; }
 };
-__device__ __forceinline__ void fo_assign_dev(const FoJob& j) {
+__global__ void __launch_bounds__(kThreads) k_fo_assign(const FoJob* jobs) {
+  const FoJob& j = jobs[blockIdx.y];
   uint32_t entries = j.hashed ? j.hmask + 1 : j.universe;
   for (uint32_t e = gtid(); e < entries; e += gstride()) {
     uint32_t f, key;
@@ -1701,7 +1670,8 @@ __device__ __forceinline__ void fo_assign_dev(const FoJob& j) {
 }
 // element -> dictionary index (+ validity bitmap, null count). Four independent elements per thread
 // keep enough loads in flight.
-__device__ __forceinline__ void fo_map_dev(const FoJob& j) {
+__global__ void __launch_bounds__(kThreads) k_fo_map(const FoJob* jobs) {
+  const FoJob& j = jobs[blockIdx.y];
   if (!j.out) return;
   uint32_t n = j.n_map_ptr ? *j.n_map_ptr : (j.n_ptr ? *j.n_ptr : j.n_imm), begin, end;
   block_range(n, &begin, &end);
@@ -1730,11 +1700,6 @@ __device__ __forceinline__ void fo_map_dev(const FoJob& j) {
     if ((threadIdx.x & 31) == 0 && nulls) atomicAdd(j.n_null, nulls);
   }
 }
-__global__ void __launch_bounds__(kThreads) k_fo_min(const FoJob* jobs) { pdl_enter(); fo_min_dev(jobs[blockIdx.y]); }
-__global__ void __launch_bounds__(kThreads) k_fo_zero(const FoJob* jobs) { pdl_enter(); fo_zero_dev(jobs[blockIdx.y]); }
-__global__ void __launch_bounds__(kThreads) k_fo_bits(const FoJob* jobs) { pdl_enter(); fo_bits_dev(jobs[blockIdx.y]); }
-__global__ void __launch_bounds__(kThreads) k_fo_assign(const FoJob* jobs) { pdl_enter(); fo_assign_dev(jobs[blockIdx.y]); }
-__global__ void __launch_bounds__(kThreads) k_fo_map(const FoJob* jobs) { pdl_enter(); fo_map_dev(jobs[blockIdx.y]); }
 
 // ---------------------------------------------------------------------------------------------
 // location dictionary: resolved per-frame attributes gathered in location order
@@ -1779,9 +1744,7 @@ struct LocLinesF {  // scan of has_line over locations (lineListOffsets, parca_r
   __device__ void total(int, uint32_t t) const { ctr_w->n_lines = t; }
 };
 // validity words of the lines ListView (null where the location has no line, arrow_v2.go:403-418)
-__device__ __forceinline__ void line_validity_dev(const Counters* ctr, const int* line_size, uint32_t* words);
-__global__ void __launch_bounds__(kThreads) k_line_validity(const Counters* ctr, const int* line_size, uint32_t* words) { pdl_enter(); line_validity_dev(ctr, line_size, words); }
-__device__ __forceinline__ void line_validity_dev(const Counters* ctr, const int* line_size, uint32_t* words) {
+__global__ void __launch_bounds__(kThreads) k_line_validity(const Counters* ctr, const int* line_size, uint32_t* words) {
   uint32_t n = ctr->n_locations;
   uint32_t nw = (n + 31) / 32;
   int lane = threadIdx.x & 31;
@@ -1793,103 +1756,11 @@ __device__ __forceinline__ void line_validity_dev(const Counters* ctr, const int
   }
 }
 // function table in function-dictionary order: filename keys for the nested dictionary
-__device__ __forceinline__ void func_keys_dev(const Counters* ctr, const uint32_t* func_order, const uint32_t* fn_file_cid, uint32_t* file_key) {
+__global__ void __launch_bounds__(kThreads) k_func_keys(const Counters* ctr, const uint32_t* func_order, const uint32_t* fn_file_cid, uint32_t* file_key) {
   uint32_t n = ctr->n_functions;
   for (uint32_t k = blockIdx.x * kThreads + threadIdx.x; k < n; k += gridDim.x * kThreads) file_key[k] = fn_file_cid[func_order[k]];
 }
-__global__ void __launch_bounds__(kThreads) k_func_keys(const Counters* ctr, const uint32_t* func_order, const uint32_t* fn_file_cid,
-                                                        uint32_t* file_key) { pdl_enter();
-  func_keys_dev(ctr, func_order, fn_file_cid, file_key);
-}
 
-// ---------------------------------------------------------------------------------------------
-// The two chains of small dependent passes (stack ranking; location / function / string dictionaries) as ONE persistent
-// kernel each: the phases are the same device functions the stand-alone kernels run, separated by a grid-wide barrier
-// (arrive on a counter, spin until everybody has). With two blocks per SM a barrier costs ~2 us, a dependent kernel launch
-// 6-9 us, and there are 5 + 21 of them. The blocks need not be co-resident from the start: nothing else on the GPU waits for
-// them, so late blocks simply arrive late. (Round 1 tried cooperative-groups grid.sync() on the full 592-block grid and
-// measured ~8 us per sync; the fix is the small grid and the bare counter.)
-__device__ __forceinline__ void grid_barrier(uint32_t* counter, uint32_t& target) {
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    target += gridDim.x;
-    __threadfence();                                   // release: this block's writes are visible before it arrives
-    atomicAdd(counter, 1u);
-    while (*(volatile uint32_t*)counter < target) { }
-    __threadfence();                                   // acquire: drops this SM's stale L1 lines
-  }
-  __syncthreads();
-}
-struct RankChainArgs {
-  StackSlot* tab; const uint32_t* claimed; Counters* ctr; uint32_t* rowbits; uint32_t* row_wprefix; uint32_t n_words;
-  const uint16_t* nframes; uint32_t* uniq_row; uint32_t* uniq_slot; uint32_t* uniq_size;
-  uint32_t* partial32; unsigned long long* partial64;
-  // tail phases (no barrier between them): per-row ListView (offset, size); frames of the unique stacks
-  uint32_t n_rows; const uint32_t* slot_of_row; int* st_offsets; int* st_sizes;
-  const unsigned long long* frames; const unsigned long long* frame_off; uint32_t n_frames_registered; uint32_t* ustream; uint32_t* loc_first;
-  uint32_t narrow;
-};
-__global__ void __launch_bounds__(kThreads) k_rank_chain(RankChainArgs a) {
-  uint32_t target = 0;
-  uint32_t* bar = &a.ctr->chain_bar[0];
-  stack_bits_dev(a.tab, a.claimed, &a.ctr->n_claimed, a.rowbits);
-  grid_barrier(bar, target);
-  { WordsF f{a.rowbits, a.row_wprefix, a.n_words, &a.ctr->n_unique}; scan_reduce_dev(f, a.partial32); grid_barrier(bar, target); scan_emit_dev(f, a.partial32, 0); }
-  grid_barrier(bar, target);
-  stack_assign_dev(a.tab, a.claimed, &a.ctr->n_claimed, a.rowbits, a.row_wprefix, a.nframes, a.uniq_row, a.uniq_slot, a.uniq_size);
-  grid_barrier(bar, target);
-  { UniqOffsetF f{a.ctr, a.ctr, a.uniq_size, a.uniq_slot, a.tab}; scan_reduce_dev(f, a.partial64); grid_barrier(bar, target); scan_emit_dev(f, a.partial64, 0); }
-  grid_barrier(bar, target);
-  rows_materialize_dev(a.n_rows, a.slot_of_row, a.tab, a.st_offsets, a.st_sizes, nullptr);
-  gather_unique_dev(a.ctr, a.uniq_row, a.slot_of_row, a.tab, a.frames, a.frame_off, a.n_frames_registered, a.ustream, a.loc_first, a.ctr, a.narrow);
-}
-struct LocChainArgs {
-  const FoJob* jobs; int j_loc, j_type, j_file;
-  Counters* ctr;
-  const uint32_t* loc_order; FrameTable ft; LocOut lo;       // LocLinesF
-  const uint32_t* fn_order; const uint32_t* fn_file_cid; uint32_t* file_key;
-  uint32_t* partial;                                         // [4][gridDim.x] block totals of the scans
-};
-__global__ void __launch_bounds__(kThreads) k_loc_chain(LocChainArgs a) {
-  uint32_t target = 0;
-  uint32_t* bar = &a.ctr->chain_bar[1];
-  const uint32_t G = gridDim.x;
-  // location index per unique-stack frame (in place over the gathered stream)
-  fo_zero_dev(a.jobs[a.j_loc]); grid_barrier(bar, target);
-  fo_bits_dev(a.jobs[a.j_loc]); grid_barrier(bar, target);
-  { FoWordsF f{a.jobs, a.j_loc}; scan_reduce_dev(f, a.partial); grid_barrier(bar, target); scan_emit_dev(f, a.partial, 0); }
-  grid_barrier(bar, target);
-  fo_assign_dev(a.jobs[a.j_loc]); grid_barrier(bar, target);
-  fo_map_dev(a.jobs[a.j_loc]);
-  // location columns + line offsets (needs loc_order from the assign phase only)
-  { LocLinesF f{a.ctr, a.ctr, a.loc_order, a.ft, a.lo}; scan_reduce_dev(f, a.partial); grid_barrier(bar, target); scan_emit_dev(f, a.partial, 0); }
-  grid_barrier(bar, target);
-  line_validity_dev(a.ctr, a.lo.line_size, a.lo.line_valid);
-  // frame_type, mapping_file, mapping_build_id, function: four independent rankings, phase by phase
-  for (int q = 0; q < 4; q++) fo_zero_dev(a.jobs[a.j_type + q]);
-  grid_barrier(bar, target);
-  for (int q = 0; q < 4; q++) fo_min_dev(a.jobs[a.j_type + q]);
-  grid_barrier(bar, target);
-  for (int q = 0; q < 4; q++) fo_bits_dev(a.jobs[a.j_type + q]);
-  grid_barrier(bar, target);
-  for (int q = 0; q < 4; q++) { FoWordsF f{a.jobs, a.j_type + q}; scan_reduce_dev(f, a.partial + q * G); }
-  grid_barrier(bar, target);
-  for (int q = 0; q < 4; q++) { FoWordsF f{a.jobs, a.j_type + q}; scan_emit_dev(f, a.partial + q * G, 0); }
-  grid_barrier(bar, target);
-  for (int q = 0; q < 4; q++) fo_assign_dev(a.jobs[a.j_type + q]);
-  grid_barrier(bar, target);
-  for (int q = 0; q < 4; q++) fo_map_dev(a.jobs[a.j_type + q]);
-  // function.filename (keys follow the function dictionary order)
-  func_keys_dev(a.ctr, a.fn_order, a.fn_file_cid, a.file_key);
-  fo_zero_dev(a.jobs[a.j_file]);
-  grid_barrier(bar, target);
-  fo_min_dev(a.jobs[a.j_file]); grid_barrier(bar, target);
-  fo_bits_dev(a.jobs[a.j_file]); grid_barrier(bar, target);
-  { FoWordsF f{a.jobs, a.j_file}; scan_reduce_dev(f, a.partial); grid_barrier(bar, target); scan_emit_dev(f, a.partial, 0); }
-  grid_barrier(bar, target);
-  fo_assign_dev(a.jobs[a.j_file]); grid_barrier(bar, target);
-  fo_map_dev(a.jobs[a.j_file]);
-}
 
 // The label column plan of the batch, checked and applied at the head of the label chain. For every labelset the batch names
 // (first_ls != kNull, recorded by k_header; in a merged batch all-reduced over the shards) a warp gives it a row of the key
@@ -1910,7 +1781,7 @@ struct LsPlanArgs {
   uint32_t plan_ord[kMaxCols];              // name ordinal of each planned column, ascending
   uint32_t* col_first[kMaxCols];            // first-row table of each planned column, by value id
 };
-__global__ void __launch_bounds__(kThreads) k_ls_plan(LsPlanArgs a) { pdl_enter();
+__global__ void __launch_bounds__(kThreads) k_ls_plan(LsPlanArgs a) {
   __shared__ uint32_t s_ord[kMaxCols];
   for (uint32_t i = threadIdx.x; i < a.n_cols; i += kThreads) s_ord[i] = a.plan_ord[i];
   __syncthreads();
@@ -2028,6 +1899,7 @@ struct ReeGroup { uint32_t type, col, param; };
 struct ReeGroups { uint32_t n; ReeGroup g[kMaxCols]; };
 
 constexpr int kReeUnroll = 4;  // 32-row sub-steps per iteration: their key loads / rank lookups are in flight together
+constexpr int kReeBlocksPerSm = 8;  // grid of the two run-end passes: they are latency-bound, so they fill every warp slot
 
 template <bool EMIT, bool MERGED, class KeyT, class K>
 __device__ __forceinline__ void ree_single(const ReeArgs& a, uint32_t c, bool has_dict, K kf) {
@@ -2195,7 +2067,7 @@ __device__ __forceinline__ void ree_kinds(const ReeArgs& a, const uint32_t* s_ki
 }
 
 template <bool EMIT, bool MERGED>
-__global__ void __launch_bounds__(kThreads) k_ree_col(ReeArgs a, ReeGroups groups) { pdl_enter();
+__global__ void __launch_bounds__(kThreads) k_ree_col(ReeArgs a, ReeGroups groups) {
   __shared__ uint32_t s_kind[64], s_krank[64];
   const ReeGroup g = groups.g[blockIdx.y];
   if (g.type == COL_KIND) {
@@ -2213,7 +2085,7 @@ __global__ void __launch_bounds__(kThreads) k_ree_col(ReeArgs a, ReeGroups group
     default: ree_single<EMIT, MERGED, long long>(a, g.col, false, KeyTs{a.ts}); break;           // COL_TS: Int64RunEndBuilder.Append
   }
 }
-__global__ void __launch_bounds__(kThreads) k_ree_scan_partials(ReeArgs a, int g, uint32_t col0) { pdl_enter();  // grid = columns col0 .., kThreads threads
+__global__ void __launch_bounds__(kThreads) k_ree_scan_partials(ReeArgs a, int g, uint32_t col0) {  // grid = columns col0 .., kThreads threads
   const uint32_t c = col0 + blockIdx.x;
   uint32_t* p = a.partial + (size_t)c * g;
   uint32_t run = 0;
@@ -2229,141 +2101,6 @@ __global__ void __launch_bounds__(kThreads) k_ree_scan_partials(ReeArgs a, int g
     if (run) a.cols[c].run_ends[run - 1] = (int)(a.row_base + a.n_rows);  // the last run ends at the (shard's last global) row count
   }
 }
-
-// ---------------------------------------------------------------------------------------------
-// Run-end encoding in ONE sweep (single aggregator; label columns and the v1 stacktrace_id / timestamp columns): a warp takes
-// tiles of 128 rows in ticket order, detects the run starts of its tile in registers, publishes the tile's count, learns how
-// many runs precede it by decoupled look-back over its predecessors' descriptors (aggregate / inclusive prefix, one 64-bit
-// word per tile, Merrill & Garland's single-pass scan), and writes run ends, final dictionary indices and validity bits
-// straight from the registers that hold the keys. Each key array is read once; there is no count pass, no partial scan.
-// The dictionary ranks are computed BEFORE this pass (their first-row tables come from k_header). The 8 kind-derived columns
-// keep the two-pass form (k_ree_col: they share one key and are almost always a single run).
-struct ReeTiles {
-  unsigned long long* desc;  // [ncols][n_tiles]: state << 62 | runs; state 0 = not yet, 1 = this tile's count, 2 = count of all tiles up to and including this one
-  uint32_t* next;            // [ncols] ticket counters
-  uint32_t n_tiles;
-};
-constexpr uint32_t kTileRows = 32 * kReeUnroll;
-constexpr unsigned long long kTileAgg = 1ull << 62, kTilePrefix = 2ull << 62;
-__device__ __forceinline__ unsigned long long ld_desc(const unsigned long long* p) {
-  unsigned long long v;
-  asm volatile("ld.volatile.global.u64 %0, [%1];" : "=l"(v) : "l"(p));
-  return v;
-}
-__device__ __forceinline__ void st_desc(unsigned long long* p, unsigned long long v) { asm volatile("st.volatile.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory"); }
-
-template <class KeyT, class K>
-__device__ __forceinline__ void ree_onepass(const ReeArgs& a, const ReeTiles& tl, uint32_t c, bool has_dict, K kf) {
-  const unsigned full = 0xFFFFFFFFu;
-  const int lane = threadIdx.x & 31;
-  const ReeCol col = a.cols[c];
-  unsigned long long* desc = tl.desc + (size_t)c * tl.n_tiles;
-  const unsigned lt = (1u << lane) - 1u;
-  uint32_t last = 0, nulls = 0;
-  for (;;) {
-    uint32_t t = 0;
-    if (lane == 0) t = atomicAdd(&tl.next[c], 1u);
-    t = __shfl_sync(full, t, 0);
-    if (t >= tl.n_tiles) break;
-    const uint32_t base = t * kTileRows;
-    KeyT key[kReeUnroll]; bool null[kReeUnroll], in[kReeUnroll], bnd[kReeUnroll];
-    unsigned m[kReeUnroll];
-    KeyT ckey = 0; bool cnull = true;  // the row before the tile
-    if (base > 0) kf.get(base - 1, ckey, cnull);
-#pragma unroll
-    for (int u = 0; u < kReeUnroll; u++) {
-      const uint32_t r = base + u * 32 + lane;
-      in[u] = r < a.n_rows; key[u] = 0; null[u] = true;
-      if (in[u]) kf.get(r, key[u], null[u]);
-    }
-    uint32_t cnt = 0;
-#pragma unroll
-    for (int u = 0; u < kReeUnroll; u++) {
-      const uint32_t r = base + u * 32 + lane;
-      KeyT pk = __shfl_up_sync(full, key[u], 1); int pn = __shfl_up_sync(full, (int)null[u], 1);
-      if (lane == 0) { pk = ckey; pn = cnull; }
-      bnd[u] = in[u] && (r == 0 || null[u] || pn || pk != key[u]);
-      m[u] = __ballot_sync(full, bnd[u]);
-      cnt += (uint32_t)__popc(m[u]);
-      ckey = __shfl_sync(full, key[u], 31); cnull = __shfl_sync(full, (int)null[u], 31);
-      const unsigned nn = __ballot_sync(full, in[u] && !null[u]);
-      if (nn) last = base + u * 32 + (32 - __clz(nn));
-      nulls += (uint32_t)__popc(__ballot_sync(full, bnd[u] && null[u]));
-    }
-    // publish this tile's count, then find how many runs precede the tile
-    if (lane == 0) st_desc(&desc[t], (t == 0 ? kTilePrefix : kTileAgg) | cnt);
-    uint32_t excl = 0;
-    if (t > 0) {
-      int j = (int)t - 1;  // lane L looks at tile j - L
-      for (;;) {
-        const int idx = j - lane;
-        unsigned long long d;
-        do { d = idx >= 0 ? ld_desc(&desc[idx]) : kTilePrefix; } while (__any_sync(full, (d >> 62) == 0ull));
-        const unsigned pm = __ballot_sync(full, (d >> 62) == 2ull);
-        const int stop = pm ? __ffs(pm) - 1 : 31;  // nearest tile that already knows its inclusive prefix
-        uint32_t v = lane <= stop ? (uint32_t)d : 0u;
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(full, v, o);
-        excl += v;
-        if (pm) break;
-        j -= 32;
-      }
-      if (lane == 0) st_desc(&desc[t], kTilePrefix | (excl + cnt));
-    }
-    // emit from the registers that still hold the tile
-    uint32_t k[kReeUnroll], stored[kReeUnroll];
-    uint32_t run = excl;
-#pragma unroll
-    for (int u = 0; u < kReeUnroll; u++) { k[u] = run + (uint32_t)__popc(m[u] & lt); run += (uint32_t)__popc(m[u]); }
-#pragma unroll
-    for (int u = 0; u < kReeUnroll; u++) {  // all dictionary lookups of the tile are issued before any is consumed
-      stored[u] = (uint32_t)key[u];
-      if (has_dict && bnd[u]) stored[u] = null[u] ? 0u : col.rank[col.hslots ? fo_hfind(col.hslots, col.hmask, (uint32_t)key[u]) : (uint32_t)key[u]];
-    }
-#pragma unroll
-    for (int u = 0; u < kReeUnroll; u++) {
-      if (bnd[u]) {
-        if (k[u] > 0) col.run_ends[k[u] - 1] = (int)(base + u * 32 + lane);  // run k starts here => run k-1 ends here
-        if (sizeof(KeyT) == 8) a.ts_vals[k[u]] = (long long)key[u]; else col.run_keys[k[u]] = stored[u];
-      }
-    }
-    if (col.validity && col.nullable) {  // validity bits of the runs emitted by one sub-step span at most two words
-      uint32_t pos = excl;
-#pragma unroll
-      for (int u = 0; u < kReeUnroll; u++) {
-        if (m[u]) {
-          const uint32_t w0 = pos >> 5;
-          const bool v = bnd[u] && !null[u];
-          unsigned m0 = __reduce_or_sync(full, (v && (k[u] >> 5) == w0) ? (1u << (k[u] & 31)) : 0u);
-          unsigned m1 = __reduce_or_sync(full, (v && (k[u] >> 5) != w0) ? (1u << (k[u] & 31)) : 0u);
-          if (lane == 0) { if (m0) atomicOr(&col.validity[w0], m0); if (m1) atomicOr(&col.validity[w0 + 1], m1); }
-        }
-        pos += (uint32_t)__popc(m[u]);
-      }
-    }
-    if (t + 1 == tl.n_tiles && lane == 0) {  // the tile with the last row closes the column
-      a.ctr->n_runs[c] = run;
-      if (run) col.run_ends[run - 1] = (int)a.n_rows;
-    }
-  }
-  if (lane == 0) {
-    if (last) atomicMax(&a.ctr->last_nonnull_plus1[c], last);
-    if (nulls) atomicAdd(&a.ctr->n_null[c], nulls);
-  }
-}
-__global__ void __launch_bounds__(kThreads) k_ree_onepass(ReeArgs a, ReeGroups groups, ReeTiles tl) {
-  const ReeGroup g = groups.g[blockIdx.y];
-  switch (g.type) {
-    case COL_LS: ree_onepass<uint32_t>(a, tl, g.col, true, KeyLs{a.ls, a.ls_rank, a.ls_keys, a.n_lscols, g.param}); break;
-    case COL_CPU: ree_onepass<uint32_t>(a, tl, g.col, true, KeyU32{a.cpu}); break;
-    case COL_TID: ree_onepass<uint32_t>(a, tl, g.col, true, KeyU32{a.tid}); break;
-    case COL_COMM: ree_onepass<uint32_t>(a, tl, g.col, true, KeyComm{a.comm}); break;
-    case COL_ORD: ree_onepass<uint32_t>(a, tl, g.col, false, KeyU32{a.ord}); break;
-    case COL_TS: ree_onepass<long long>(a, tl, g.col, false, KeyTs{a.ts}); break;
-    default: break;  // the kind-derived group goes through k_ree_col
-  }
-}
-
 
 // ---------------------------------------------------------------------------------------------
 // v1 schema: device-resident store of known stacks — the `stacks` LRU of the reference
